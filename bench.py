@@ -2,11 +2,15 @@
 """Benchmark of the PanFusion denoise hot path (BASELINE.json metric: denoise-steps/sec, 512x1024 pano + 8x512^2
 views, CFG batch 2, bf16, 50-step DDIM schedule).
 
-    python bench.py --gpus N --steps K --warmup W            # this repo's sm_100a path
+    python bench.py --gpus N --steps K --warmup W            # this repo's sm_90a (H100) path
     python bench.py --impl reference --steps K --warmup W     # the reference algorithm's CPU path (oracle port)
 
 One "step" = one iteration of the reference loop models/pano/PanFusion.py:146-162: rotate, CFG-batched
 MultiViewBaseModel.forward (7 EPPA fusions), CFG combine, two DDIM updates. Prints ONE JSON line (rank 0).
+--dump-outputs DIR additionally writes, after the timed steps, the view and panorama latents of the last timed step
+as DIR/latents.npy and DIR/pano_latents.npy (float32), in the frame the loop holds them after that step (what
+PanFusionSampler.finish(rotate_back=False) returns; the panorama is not rotated back): with the same arguments the
+inputs are the same seeded tensors, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -64,11 +68,12 @@ def peaks():
     if p.exists():
         d = json.loads(p.read_text())
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sust=d["bf16_tflops_sustained"], src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, src="fallback")
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s; not measured here
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries every 100 ms)."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -192,7 +197,7 @@ def run_b200(args):
     cond = inp["pano_layout_cond"].to(dev) if "pano_layout_cond" in inp else None
     sampler.start(lat, pano, prompt, pano_prompt, inp["cams"], pano_layout_cond=cond)
     if args.profile_one_step:
-        # ncu --profile-from-start off: tables/weights warmed by 4 eager steps, then exactly one step is profiled
+        # a profiler started with capture disabled: tables/weights warmed by 4 eager steps, then exactly one step is profiled
         sampler.use_cuda_graph = False
         for i in range(4):
             sampler.step(i)
@@ -224,6 +229,9 @@ def run_b200(args):
         e1.record()
         torch.cuda.synchronize()
     ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        lat_out, pano_out = sampler.finish(rotate_back=False)
+        dump_outputs(args.dump_outputs, latents=lat_out, pano_latents=pano_out)
     if world > 1:
         t = torch.tensor([ms], device=dev)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -293,7 +301,8 @@ def run_b200(args):
                        "view_latent": list(wl["pers_hw"]), "weights": "random-init SD-2 architecture (seeded)",
                        "parallelism": parallelism,
                        "cuda_graph": not args.no_graph,
-                       "l2": "working set (3.4 GB weights + activations per step) exceeds the 126 MB L2; no flush needed"},
+                       "l2": "working set (3.4 GB weights + activations per step) exceeds the 50 MB L2; no flush needed"},
+            "gpu": torch.cuda.get_device_name(dev),
             "clocks": clk.summary(),
             "e2e": {"value": round(e2e_sps, 4), "unit": "steps/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
             "eppa_tables_mb": round(model.cp_blocks_mid.tables.nbytes() / 2 ** 20, 1),  # all 4 rotation phases, resident form
@@ -316,23 +325,26 @@ def run_b200(args):
         print(json.dumps(out))
 
 
-def _ncu_traffic():
-    """DRAM bytes per launch of the resampling kernels from the committed `ncu --set full` captures
-    (profiles/resample_traffic.json: dram__bytes_read.sum + dram__bytes_write.sum); absent -> null."""
-    f = ROOT / "profiles" / "resample_traffic.json"
-    return json.loads(f.read_text()) if f.exists() else {}
+def dump_outputs(out_dir, **arrays):
+    """Write each array as <out_dir>/<name>.npy in float32 (the whole tensor: these outputs are well under 64 MB)."""
+    import numpy as np
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        assert a.nbytes <= 64 << 20, (name, a.nbytes)
+        np.save(d / f"{name}.npy", a)
 
 
 def micro_rooflines(dev, pk):
     """Isolated timings of the kernels the north star names. Each kernel is launched 20x inside ONE captured CUDA
     graph (no Python between launches), timed with CUDA events around graph replays; the launches rotate over
-    enough distinct input/output buffers that consecutive launches never touch the same bytes within 126 MB of L2."""
+    enough distinct input/output buffers that consecutive launches never touch the same bytes within 50 MB of L2."""
     import numpy as np
     from panfusion_b200 import geometry, ops
     from panfusion_b200.engine import taps3x3
     from panfusion_b200.packing import pack_conv3x3
     res = {}
-    traffic = _ncu_traffic()
     ev = lambda: torch.cuda.Event(enable_timing=True)
 
     def timeit(fns, launches=20, reps=5):
@@ -355,11 +367,8 @@ def micro_rooflines(dev, pk):
         return a.elapsed_time(b) / (reps * launches)
 
     def hbm_entry(name, ms, alg, note):
-        t = traffic.get(name)
         res[name] = {"bound": "hbm", "ms": round(ms, 4), "algorithmic_bytes": alg, "achieved": round(alg / ms / 1e6, 1),
-                     "peak": pk["hbm"], "unit": "GB/s", "frac": round(alg / ms / 1e6 / pk["hbm"], 4),
-                     "traffic": t["dram_bytes"] if t else None, "traffic_source": t["source"] if t else None,
-                     "shape": note}
+                     "peak": pk["hbm"], "unit": "GB/s", "frac": round(alg / ms / 1e6 / pk["hbm"], 4), "shape": note}
 
     th16 = torch.tensor(np.tile(np.arange(8) * 45.0, 2), dtype=torch.float32)
     fov16, phi16 = torch.full((16,), 90.0), torch.zeros(16)
@@ -494,7 +503,7 @@ def _oracle_model(layout_cond: bool = False):
 class _OracleLoop:
     """The reference's sampling loop (models/pano/PanFusion.py:146-162: rotate -> CFG-batched
     MultiViewBaseModel.forward -> CFG combine -> 2x DDIM update) on the host cores, through the oracle port, on the
-    benchmark workload itself (same views / latent sizes / CFG batch / cameras / guidance as the B200 arm)."""
+    benchmark workload itself (same views / latent sizes / CFG batch / cameras / guidance as the GPU arm)."""
 
     def __init__(self, workload):
         from oracle import sampler as osamp
@@ -535,16 +544,17 @@ def cpu_baseline(workload, budget_s=30.0):
 def run_reference(args):
     """`--impl reference`: the reference algorithm's own CPU path (oracle port; diffusers/xformers/kornia are not
     installable offline, SURVEY.md §8c) on the usable host cores, REAL steps of the benchmark workload: one warm-up
-    step, then as many timed steps as fit `--ref-budget` seconds (at least 2, at most --steps). `steps` / `warmup` in
-    the JSON line are the counts actually run. Rank 0 only."""
+    step, then exactly --steps timed steps (about a minute each at C2 on 16 cores). Rank 0 only."""
     if int(os.environ.get("RANK", 0)) != 0:
         return
     wl = WORKLOADS[args.workload]
     cores = host_threads()
     loop = _OracleLoop(args.workload)
-    t_warm = loop.step()
-    n_timed = max(2, min(args.steps, int(args.ref_budget / max(t_warm, 1e-3))))
+    loop.step()  # warm-up
+    n_timed = args.steps
     times = [loop.step() for _ in range(n_timed)]
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, latents=loop.lat, pano_latents=loop.pano)
     per = sum(times) / n_timed
     val = round(1.0 / per, 5)
     sample = (f"{n_timed} full denoise steps of this workload after 1 warm-up step (rotate + CFG-batched forward + combine "
@@ -573,10 +583,13 @@ def main():
     ap.add_argument("--skip-micro", action="store_true", help="skip the isolated kernel rooflines")
     ap.add_argument("--skip-image", action="store_true", help="skip the cold / warm whole-image latency leg")
     ap.add_argument("--cpu-budget", type=float, default=30.0)
-    ap.add_argument("--ref-budget", type=float, default=240.0,
-                    help="--impl reference: seconds of TIMED reference steps (at least 2 steps are always run)")
-    ap.add_argument("--profile-one-step", action="store_true", help="for ncu --profile-from-start off: profile one eager step")
+    ap.add_argument("--profile-one-step", action="store_true",
+                    help="run one eager step between cudaProfilerStart/Stop (for a range-limited profiler capture)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the latents of the last timed step to DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":
         run_reference(args)

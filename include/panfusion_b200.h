@@ -1,5 +1,5 @@
 /*
- * panfusion_b200 — C ABI of the B200 (sm_100a) denoise hot path of PanFusion.
+ * panfusion_b200 — C ABI of the H100 (sm_90a) denoise hot path of PanFusion.
  *
  * Every entry point takes plain device pointers, sizes and a CUDA stream (cudaStream_t passed as void*).
  * The caller (PyTorch on the host side) owns every buffer; the library keeps no hidden state except a
@@ -21,7 +21,7 @@ extern "C" {
 #define PF_OK 0
 #define PF_ERR_INVALID (-1)     /* bad argument (message in pf_last_error) */
 #define PF_ERR_CUDA (-2)        /* CUDA runtime / driver failure */
-#define PF_ERR_UNSUPPORTED (-3) /* shape / dtype not supported by the sm_100a kernels */
+#define PF_ERR_UNSUPPORTED (-3) /* shape / dtype not supported by the sm_90a kernels */
 
 typedef enum { PF_F32 = 0, PF_F16 = 1, PF_BF16 = 2 } pf_dtype;
 
@@ -29,7 +29,7 @@ typedef enum { PF_F32 = 0, PF_F16 = 1, PF_BF16 = 2 } pf_dtype;
  * external/Perspective_and_Equirectangular/utils.py:15); here: return code + message. */
 const char* pf_last_error(void);
 int pf_version(void);
-/* returns 0 iff the current device is compute capability 10.x (B200); the library has no other path */
+/* returns 0 iff the current device is compute capability 9.0 (H100); the library has no other path */
 int pf_check_device(void);
 
 /* ------------------------------------------------------------------------------------------------
@@ -74,7 +74,7 @@ int pf_p2e(const void* src, void* dst, uint8_t* mask, int dtype, int B, int C, i
            const double* cams, int cam_stride, int mode, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Tap-GEMM (tcgen05 / TMEM / TMA): the one dense-contraction engine behind nn.Linear (K8, K10) and the
+ * Tap-GEMM (wgmma / TMA): the one dense-contraction engine behind nn.Linear (K8, K10) and the
  * 3x3 / 1x1 convolutions (K9, K11) of the UNet walk in models/pano/MVGenModel.py:85-295.
  *
  *   acc[m, n] = sum_{t < num_taps} sum_{k < Kc} A[m + tap_off[t], k] * B[n, t*Kc + k]      (fp32 accumulate)
@@ -153,7 +153,7 @@ int pf_gemm_splitk_plan(const pf_gemm_args* args);
 int pf_gemm_pick_block_n(int N, int act);
 
 /* ------------------------------------------------------------------------------------------------
- * Flash attention forward (tcgen05): out = softmax(q k^T * scale + bias) v, fp32 softmax / accumulation.
+ * Flash attention forward (wgmma): out = softmax(q k^T * scale + bias) v, fp32 softmax / accumulation.
  * Replaces xformers.ops.memory_efficient_attention at models/modules/transformer.py:71 (EPPA: head_dim 32,
  * additive fp32 bias shared by every head — transformer.py:68 materialises it per head, this never does) and the
  * bmm-softmax-bmm of the diffusers attention blocks walked at models/pano/MVGenModel.py:104,116,185,190,227,241
@@ -233,9 +233,9 @@ int pf_conv_prep(const void* x, void* out, int dtype, int N, int H, int W, int C
  *   statistics over the image circularly extended by circ_stats columns (duplicated columns count twice), applied with
  *   gamma / beta (+ SiLU) while building the conv_prep layout (circ, up, phases, halo as in pf_conv_prep).
  * The kernel holds a per-image barrier between the statistics and the apply phase (the source is re-read from L2), so its
- * grid is capped at 148 CTAs of <= 512 threads — two such launches (the two UNet branches' streams) are always co-resident.
+ * grid is capped at one CTA of <= 512 threads per SM — two such launches (the two UNet branches' streams) are always co-resident.
  * schedule: 1 = that fused launch, 2 = two launches (statistics with one CTA per slab, then the apply pass: no barrier, many
- * more CTAs per image — measured faster at every batch size of the denoise step), 0 = default (two launches unless
+ * more CTAs per image), 0 = default (two launches unless
  * PF_GN_FUSED_MIN_N says otherwise). Same bits either way.
  * ws: pf_gn_prep_ws_floats(N, groups) floats of scratch; sync: 3*N ints that are ZERO on entry (restored to zero by the
  * kernel; concurrent launches need distinct slots). The partition of every sum depends on H*W only, never on N: results are

@@ -41,6 +41,10 @@ def _report(name, ref, mine):
     return err
 
 
+def _trunc10(a):
+    return (np.ascontiguousarray(a, dtype=np.float32).view(np.uint32) & np.uint32(0xFFFFFC00)).view(np.float32)
+
+
 def golden_c2(ref):
     """BASELINE configs[1], the benchmarked configuration: SD-2 widths, 8 horizon views 64x64 + pano 64x128, the CFG
     pair (b = 2, prompts [null; text]) — ONE reference MultiViewBaseModel.forward (MVGenModel.py:38-297) on CPU."""
@@ -51,7 +55,9 @@ def golden_c2(ref):
     rs, rp_ = model_r(**inp)
     t1 = time.time()
     print(f"  [c2] reference forward {t1 - t0:.1f}s", flush=True)
-    np.savez_compressed(OUT / "mvgen_c2.npz", sample=rs.numpy(), pano_sample=rp_.numpy())
+    # the 10 low significand bits are cleared (|change| <= 7.5e-5 of max|ref|, far below the fp16 gate of 4e-3) so that
+    # the compressed fixture stays under 1 MB
+    np.savez_compressed(OUT / "mvgen_c2.npz", sample=_trunc10(rs.numpy()), pano_sample=_trunc10(rp_.numpy()))
     model_o = synth.build_model(om.MultiViewBaseModel, cfg, seed=0)
     model_o.load_state_dict(model_r.state_dict())
     del model_r

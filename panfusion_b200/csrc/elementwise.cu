@@ -379,7 +379,7 @@ extern "C" int pf_conv_in(const float* x, const float* w, const float* bias, voi
   PF_CHECK_ARG(act == PF_ACT_NONE || act == PF_ACT_SILU, "pf_conv_in: act must be none or silu");
   const long long total = (long long)N * H * ((W & 3) ? W : W / 4) * (Cout / 8);
   long long want = (total + 255) / 256;
-  const unsigned blocks = (unsigned)(want < 148 * 4 ? want : 148 * 4);  // persistent-ish: weights staged once per CTA
+  const unsigned blocks = (unsigned)(want < sm_count() * 4 ? want : sm_count() * 4);  // persistent-ish: weights staged once per CTA
   const size_t smem = ((size_t)Cin * 9 * Cout + Cout) * sizeof(float);
   PF_CHECK_ARG(smem <= 200 * 1024, "pf_conv_in: Cin*9*Cout too large for shared memory");
   cudaStream_t st = static_cast<cudaStream_t>(stream);

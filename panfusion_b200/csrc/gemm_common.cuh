@@ -1,4 +1,4 @@
-// Shared declarations of the tap-GEMM kernels (gemm_persist.cu, gemm_tcgen05.cu).
+// Shared declarations of the tap-GEMM kernel (gemm_wgmma.cu).
 #pragma once
 #include "pf_common.cuh"
 
@@ -62,7 +62,5 @@ __device__ __forceinline__ void ln_row_coeffs(const GemmKernelParams& p, long lo
 __host__ __device__ constexpr int gemm_stage_bytes(int block_n) {
   return GEMM_BLOCK_M * GEMM_BLOCK_K * 2 + block_n * GEMM_BLOCK_K * 2;
 }
-
-int launch_gemm_persistent(const pf_gemm_args* a, const GemmKernelParams& kp, int bn, bool epi_tma, cudaStream_t st);
 
 }  // namespace pf

@@ -210,7 +210,7 @@ __global__ void __launch_bounds__(256) conv_prep_kernel(const PrepParams p) {
 // ------------------------------------------------------------------------------------------------
 // gn_prep: GroupNorm statistics + apply (+SiLU) + conv_prep layout in ONE launch (pf_gn_prep).
 //
-// grid = (chunks, G) with chunks * G <= GNP_MAX_CTAS, so that every CTA of the launch (and of one more such launch on
+// grid = (chunks, G) with chunks * G <= the SM count, so that every CTA of the launch (and of one more such launch on
 // the other branch's stream) is co-resident: the kernel contains a per-image barrier. CTA (c, y) serves images
 // y, y + G, ... in turn. The statistics are accumulated per SLAB — a fixed partition of the image into `slabs` pixel
 // ranges that depends on the image size ONLY — and the slabs are summed in slab order; how many slabs a CTA owns (few
@@ -223,7 +223,6 @@ __global__ void __launch_bounds__(256) conv_prep_kernel(const PrepParams p) {
 // sync[3n .. 3n+2] = {arrivals, flag, departures}: all zero on entry and restored to zero by the last CTA to leave.
 // ------------------------------------------------------------------------------------------------
 constexpr int GNP_MAX_SLABS = 64;  // upper bound of the statistics partition of one image (fixed by its size)
-constexpr int GNP_MAX_CTAS = 148;  // one CTA per SM; two such launches (2 CTAs of <= 512 threads per SM) stay co-resident
 
 __device__ __forceinline__ int ld_acquire_s32(const int* p) {
   int v;
@@ -701,10 +700,8 @@ extern "C" int pf_gn_prep(const void* x1, int ld1, int C1, const void* x2, int l
   const int threads = vecs * ppi;
   const size_t smem = 2 * (size_t)C * ppi * sizeof(float);  // <= 32 KB
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // Default: TWO launches — statistics with one CTA per slab, then the apply pass with up to 64 CTAs per image. Measured on
-  // B200 (C2 step): 37.8 steps/s against 37.3 with the single fused launch even at 16 images per call, and 7.6 vs 8+ ms for
-  // a rank's 1-image panorama branch: the barrier's latency and the grid capped for co-residency cost more than the second
-  // launch. The fused schedule stays available (schedule = 1, or PF_GN_FUSED_MIN_N=<batch size from which to use it>).
+  // Default: TWO launches — statistics with one CTA per slab, then the apply pass with up to 64 CTAs per image: the
+  // barrier's latency and the grid capped for co-residency cost more than the second launch. The fused schedule stays available (schedule = 1, or PF_GN_FUSED_MIN_N=<batch size from which to use it>).
   static const int fused_min_n = [] {
     const char* e = getenv("PF_GN_FUSED_MIN_N");
     return e ? atoi(e) : (1 << 30);
@@ -712,11 +709,13 @@ extern "C" int pf_gn_prep(const void* x1, int ld1, int C1, const void* x2, int l
   PF_CHECK_ARG(schedule >= 0 && schedule <= 2, "pf_gn_prep: schedule must be 0 (auto), 1 (fused) or 2 (two launches)");
   if (schedule == 1 || (schedule == 0 && N >= fused_min_n)) {
     // CTAs per image: the largest divisor of `slabs` that keeps the grid co-resident
-    const int cap = GNP_MAX_CTAS / (N < GNP_MAX_CTAS ? N : GNP_MAX_CTAS) > 0 ? GNP_MAX_CTAS / (N < GNP_MAX_CTAS ? N : GNP_MAX_CTAS) : 1;
+    // one CTA per SM: two such launches (2 CTAs of <= 512 threads per SM) stay co-resident
+    const int max_ctas = sm_count();
+    const int cap = max_ctas / (N < max_ctas ? N : max_ctas) > 0 ? max_ctas / (N < max_ctas ? N : max_ctas) : 1;
     int chunks = 1;
     for (int d = 1; d <= slabs && d <= cap; ++d)
       if (slabs % d == 0) chunks = d;
-    const int gy = N < GNP_MAX_CTAS / chunks ? N : GNP_MAX_CTAS / chunks;
+    const int gy = N < max_ctas / chunks ? N : max_ctas / chunks;
     dim3 grid(chunks, gy);
     if (dtype == PF_BF16) launch_pdl(gn_prep_kernel<true, 0>, grid, dim3(threads), smem, st, p);
     else launch_pdl(gn_prep_kernel<false, 0>, grid, dim3(threads), smem, st, p);
@@ -746,7 +745,7 @@ extern "C" int pf_layernorm(const void* x, int ldx, void* out, int ldo, int dtyp
   PF_CHECK_ARG(!pe || pe_rows > 0, "pf_layernorm: pe_rows must be positive");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   int blocks = (T + 7) / 8;
-  if (blocks > 148 * 8) blocks = 148 * 8;  // warps loop over tokens (affine parameters stay in registers)
+  if (blocks > sm_count() * 8) blocks = sm_count() * 8;  // warps loop over tokens (affine parameters stay in registers)
   const uint16_t* xi = static_cast<const uint16_t*>(x);
   uint16_t* xo = static_cast<uint16_t*>(out);
   const int rounds = (C / 8 + 31) / 32;

@@ -30,6 +30,19 @@ bool pdl_enabled() {
   return on;
 }
 
+int sm_count() {
+  static const int n = [] {
+    int dev = 0, v = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        v <= 0) {
+      cudaGetLastError();
+      v = 132;
+    }
+    return v;
+  }();
+  return n;
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -104,8 +117,8 @@ int pf_check_device(void) {
   cudaDeviceProp p;
   e = cudaGetDeviceProperties(&p, dev);
   if (e != cudaSuccess) return pf::check_cuda(e, "cudaGetDeviceProperties");
-  if (p.major != 10) {
-    pf::set_error("device %s is sm_%d%d; panfusion_b200 only has sm_100a kernels", p.name, p.major, p.minor);
+  if (p.major != 9 || p.minor != 0) {
+    pf::set_error("device %s is sm_%d%d; panfusion_b200 only has sm_90a kernels", p.name, p.major, p.minor);
     return PF_ERR_UNSUPPORTED;
   }
   return PF_OK;

@@ -1,7 +1,6 @@
-// panfusion_b200 — shared device/host helpers for the sm_100a kernels.
-// PTX wrappers for mbarrier, TMA (cp.async.bulk[.tensor]) and tcgen05 (UMMA + TMEM).
-// Descriptor bit layouts follow the PTX ISA "tcgen05 matrix descriptors" tables
-// (cross-checked against cute/arch/mma_sm100_desc.hpp field comments).
+// panfusion_b200 — shared device/host helpers for the sm_90a kernels.
+// PTX wrappers for mbarrier, TMA (cp.async.bulk[.tensor]) and wgmma (warpgroup MMA, accumulators in registers).
+// Descriptor bit layouts follow the PTX ISA "Matrix Descriptor Format" table of the wgmma section.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -20,6 +19,7 @@ namespace pf {
 void set_error(const char* fmt, ...);
 int  check_cuda(cudaError_t e, const char* what);
 bool pdl_enabled();  // env PF_PDL=1 (default off), pf_api.cu
+int  sm_count();     // SMs of the current device (cached; 132 on an H100 SXM when no device can be queried)
 
 #define PF_CHECK_ARG(cond, ...)                      \
   do {                                               \
@@ -79,15 +79,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug must surface as a launch failure (trap), never as a hung GPU.
+// Bounded wait: a protocol bug must surface as a launch failure (trap), never as a hung GPU. No printf here: a function
+// call in a kernel makes ptxas serialize its wgmma pipeline.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) {  // ~2 s at 2 GHz
-      printf("pf: mbarrier wait timeout (block %d,%d thread %d)\n", blockIdx.x, blockIdx.y, threadIdx.x);
-      __trap();
-    }
+    if (clock64() - t0 > 4000000000LL) __trap();  // ~2 s at 2 GHz
   }
 }
 
@@ -131,145 +129,31 @@ __device__ __forceinline__ void bulk_load_1d(void* dst, const void* src, uint32_
       : "memory");
 }
 
-// ---- tcgen05 / TMEM ---------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
+// ---- wgmma (sm_90a warpgroup MMA) -------------------------------------------------------------
+// All four warps of a warpgroup execute these together. fence: orders register accesses to the accumulators before
+// the next wgmma; commit: closes a group of issued wgmma; wait<N>: until at most N groups are still in flight.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], bf16/fp16 inputs, fp32 accumulate, issued by ONE thread.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 16 consecutive 32-bit columns: thread t of the warp gets lane (base_lane + t)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-      "%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-      "%15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
+// keeps the compiler from moving accumulator reads/writes across the asynchronous wgmma
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// registers -> TMEM, 32 lanes x 32 consecutive columns (mirror of tmem_ld32)
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-        "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]),
-        "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]),
-        "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ---- CTA-pair (cta_group::2) variants: two CTAs of a cluster issue ONE MMA of M = 256 ---------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// both CTAs issue their own loads; the transaction bytes land on the LEADER CTA's mbarrier (peer bit cleared)
-__device__ __forceinline__ void tma_load_2d_2sm(void* dst, const CUtensorMap* t, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-      "[%2];" ::"r"(smem_u32(dst)),
-      "l"(t), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on the same-offset mbarrier of BOTH CTAs once the pair's MMAs have retired
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"((uint16_t)3)
-      : "memory");
-}
-
-// Instruction descriptor, kind::f16: fp32 accumulate, A/B both `fmt` (0 = f16, 1 = bf16).
-//   [4,6) c_format=1(F32)  [7,10) a_format  [10,13) b_format  [15] a_major  [16] b_major (0 = K-major)
-//   [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_f16(int fmt, int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (uint32_t(fmt) << 7) | (uint32_t(fmt) << 10) | (uint32_t(a_mn_major) << 15) |
-         (uint32_t(b_mn_major) << 16) | (uint32_t(N >> 3) << 17) | (uint32_t(M >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor.
-//   [0,14) start>>4  [16,30) LBO>>4  [32,46) SBO>>4  [46,48) version=1 (sm_100)  [61,64) layout type
-//   layout type: 0 none, 2 = 128B swizzle, 4 = 64B swizzle, 6 = 32B swizzle
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint32_t layout_type) {
+// Shared-memory matrix descriptor of wgmma (sm_90).
+//   [0,14) start>>4  [16,30) LBO>>4  [32,46) SBO>>4  [49,52) base offset (0: tiles are swizzle-pattern aligned)
+//   [62,64) layout type: 0 none, 1 = 128B swizzle, 2 = 64B swizzle, 3 = 32B swizzle
+// K-major operands: SBO = bytes between 8-row groups, LBO unused; a 16-element K step inside a swizzle row is +32 B.
+// MN-major operands: SBO = bytes between 8-row groups along K, LBO = bytes between swizzle atoms along MN.
+__device__ __forceinline__ uint64_t make_wgmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
+                                                    uint32_t layout_type) {
   return uint64_t((saddr & 0x3FFFFu) >> 4) | (uint64_t(lbo_bytes >> 4) << 16) | (uint64_t(sbo_bytes >> 4) << 32) |
-         (uint64_t(1) << 46) | (uint64_t(layout_type) << 61);
+         (uint64_t(layout_type) << 62);
 }
 
 // ---- small numeric helpers -----------------------------------------------------------------
@@ -315,7 +199,7 @@ __device__ __forceinline__ float2 unpack2(uint32_t w) {
 
 // ---- programmatic dependent launch (PDL) -----------------------------------------------------------------
 // A denoise step is ~1000 short kernels; with plain stream order each one pays the predecessor's drain, the launch
-// latency and its own on-chip prologue (barrier init, TMEM allocation, descriptor prefetch) back to back. Kernels
+// latency and its own on-chip prologue (barrier init, descriptor prefetch) back to back. Kernels
 // launched through launch_pdl() may become resident as soon as every CTA of the predecessor has STARTED
 // (pdl_launch_dependents() is the first instruction), run their prologue, and block in pdl_wait() until the
 // predecessor grid has completed and its memory is visible. Rule: a kernel launched with launch_pdl() must execute
@@ -324,7 +208,7 @@ __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepc
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // MUFU wrappers without the denormal range fix-ups nvcc wraps around expf / division (2 FSETP + FSEL + 3 FMUL per
-// call — the GEGLU epilogue was issue-bound on them, profiles/gemm_geglu_r01_summary.txt): results feed 16-bit stores.
+// call — the GEGLU epilogue evaluates one erf-GELU per output): results feed 16-bit stores.
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -357,60 +241,11 @@ __device__ __forceinline__ float gelu_erf_f(float x) {
   return fmaf(hx, erf_as_f(x * 0.70710678118654752440f), hx);
 }
 
-// ---- packed fp32x2 arithmetic (sm_100: FFMA2 / FMUL2 / FADD2 — two IEEE fp32 operations per issued instruction) ----------
-// The GEGLU epilogue is ISSUE-bound (one erf-GELU per output element): evaluating two neighbouring columns per instruction
-// halves its FMA-pipe instruction count. Each lane rounds exactly like the scalar instruction, so results are bit-identical.
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pack_f2(float a, float b) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-  return r;
-}
-__device__ __forceinline__ void unpack_f2(f32x2 v, float& a, float& b) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
-}
-__device__ __forceinline__ f32x2 fma_f2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ f32x2 mul_f2(f32x2 a, f32x2 b) {
-  f32x2 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ f32x2 add_f2(f32x2 a, f32x2 b) {
-  f32x2 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-// (a0 + ba0) * gelu(g0 + bg0), (a1 + ba1) * gelu(g1 + bg1): the operation sequence of gelu_erf_f / erf_as_f, two lanes wide
+// (a0 + ba0) * gelu(g0 + bg0), (a1 + ba1) * gelu(g1 + bg1) for two neighbouring GEGLU columns
 __device__ __forceinline__ void geglu_pair(float a0, float a1, float g0, float g1, float ba0, float ba1, float bg0, float bg1,
                                            float& o0, float& o1) {
-  const f32x2 x = add_f2(pack_f2(g0, g1), pack_f2(bg0, bg1));
-  const f32x2 val = add_f2(pack_f2(a0, a1), pack_f2(ba0, ba1));
-  const f32x2 xs = mul_f2(x, pack_f2(0.70710678118654752440f, 0.70710678118654752440f));
-  float xs0, xs1;
-  unpack_f2(xs, xs0, xs1);
-  const float ax0 = fabsf(xs0), ax1 = fabsf(xs1);
-  const f32x2 ax = pack_f2(ax0, ax1);
-  float d0, d1;
-  unpack_f2(fma_f2(pack_f2(0.3275911f, 0.3275911f), ax, pack_f2(1.0f, 1.0f)), d0, d1);
-  const f32x2 t = pack_f2(rcp_approx(d0), rcp_approx(d1));
-  f32x2 p = fma_f2(pack_f2(1.061405429f, 1.061405429f), t, pack_f2(-1.453152027f, -1.453152027f));
-  p = fma_f2(p, t, pack_f2(1.421413741f, 1.421413741f));
-  p = fma_f2(p, t, pack_f2(-0.284496736f, -0.284496736f));
-  p = fma_f2(p, t, pack_f2(0.254829592f, 0.254829592f));
-  float e0, e1;
-  unpack_f2(mul_f2(ax, mul_f2(ax, pack_f2(-1.4426950408889634f, -1.4426950408889634f))), e0, e1);
-  const f32x2 ex = pack_f2(ex2_approx(e0), ex2_approx(e1));
-  // r = fma(-p*t, ex, 1)
-  const f32x2 npt = mul_f2(mul_f2(p, pack_f2(-1.0f, -1.0f)), t);
-  float r0, r1;
-  unpack_f2(fma_f2(npt, ex, pack_f2(1.0f, 1.0f)), r0, r1);
-  const f32x2 erfv = pack_f2(copysignf(r0, xs0), copysignf(r1, xs1));
-  const f32x2 hx = mul_f2(x, pack_f2(0.5f, 0.5f));
-  unpack_f2(mul_f2(val, fma_f2(hx, erfv, hx)), o0, o1);
+  o0 = (a0 + ba0) * gelu_erf_f(g0 + bg0);
+  o1 = (a1 + ba1) * gelu_erf_f(g1 + bg1);
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

@@ -297,7 +297,7 @@ static int launch_resample(const void* src, void* dst, uint8_t* mask, int B, int
     tile_px = (tile_px + 3) & ~3;
     const int qpt = (tile_px + 4 * STG_THREADS - 1) / (4 * STG_THREADS);
     // exactly ONE wave of co-resident CTAs (2 per SM) when the problem allows it
-    int ctas_per_bt = (148 * 2) / (B * tiles);
+    int ctas_per_bt = (sm_count() * 2) / (B * tiles);
     if (ctas_per_bt < 1) ctas_per_bt = 1;
     int ch_per_cta = (C + ctas_per_bt - 1) / ctas_per_bt;
     ch_per_cta = ((ch_per_cta + ch_per_stage - 1) / ch_per_stage) * ch_per_stage;
@@ -330,10 +330,10 @@ static int launch_resample(const void* src, void* dst, uint8_t* mask, int B, int
     int ch_per_stage = (int)((48 * 1024) / plane_bytes);
     if (ch_per_stage < 1) ch_per_stage = 1;
     if (ch_per_stage > 16) ch_per_stage = 16;
-    // enough CTAs to fill 148 SMs x 2, but long enough channel runs to amortise the fp64 grid math
+    // enough CTAs to fill every SM twice, but long enough channel runs to amortise the fp64 grid math
     int ch_per_cta = C;
-    // exactly ONE wave of co-resident CTAs (2 per SM): a 3 % overshoot of the 296 slots costs a whole second wave
-    const int want_ctas = 148 * 2;
+    // exactly ONE wave of co-resident CTAs (2 per SM): a small overshoot of those slots costs a whole second wave
+    const int want_ctas = sm_count() * 2;
     int ctas_per_b = want_ctas / B;
     if (ctas_per_b < 1) ctas_per_b = 1;
     ch_per_cta = (C + ctas_per_b - 1) / ctas_per_b;
@@ -364,7 +364,7 @@ static int launch_resample(const void* src, void* dst, uint8_t* mask, int B, int
   int ch_per_slice = C;
   {
     const long long blocks_xy = (long long)((dplane + 255) / 256) * B;
-    int slices = (int)((148LL * 8 + blocks_xy - 1) / blocks_xy);
+    int slices = (int)(((long long)sm_count() * 8 + blocks_xy - 1) / blocks_xy);
     if (slices < 1) slices = 1;
     if (slices > C) slices = C;
     ch_per_slice = (C + slices - 1) / slices;

@@ -6,7 +6,7 @@ Same constructor, sub-module / parameter names (`transformer.attn1.{to_q,to_k,to
 unchanged. What changes is the execution: the correspondence bias and the spherical PE come from cached
 per-camera tables built by two CUDA kernels (csrc/eppa_tables.cu) instead of the one-hot/grid_sample/blur
 pipeline of models/pano/utils.py:10-106, the bias is never repeated per head (transformer.py:68), and both
-attention directions run as tcgen05 flash-attention launches over one fused Q/K/V projection per token set.
+attention directions run as wgmma flash-attention launches over one fused Q/K/V projection per token set.
 """
 from __future__ import annotations
 

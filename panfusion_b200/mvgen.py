@@ -3,7 +3,7 @@
 Same constructor `(unet, pano_unet, pers_cn=None, pano_cn=None, pano_pad=True)`, same attributes (`unet`,
 `pano_unet`, `cp_blocks_encoder`, `cp_blocks_mid`, `cp_blocks_decoder`, `trainable_parameters`), same forward
 signature and return value. The UNets are consumed by attribute walk exactly like the reference does, but only to
-READ their parameters once (engine.UNetPack); every block then runs as hand-written sm_100a kernels on
+READ their parameters once (engine.UNetPack); every block then runs as hand-written sm_90a kernels on
 channels-last 16-bit activations. There is no PyTorch fallback: without a CUDA device / the built library the
 forward raises.
 """

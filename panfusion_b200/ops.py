@@ -28,11 +28,10 @@ def _st():
     return C.c_void_p(_lib.stream_ptr())
 
 
-# per-shape tile choice measured on B200 by scripts/tune_gemm.py: (M, N, Kc, taps) -> block_n
+# optional per-shape tile choice measured by scripts/tune_gemm.py: (M, N, Kc, taps) -> block_n (absent: pf_gemm_pick_block_n)
 GEMM_LOG = None
-# Split-K (pf_gemm_splitk_plan: only skinny deep-K problems — <= 74 output tiles, >= 64 K-slabs, i.e. the 8x8 / 16x16-level
-# convolutions of a small batch). Measured on B200: one rank of the 8-GPU layout 10.85 -> 9.82 ms per step, its 1-image
-# panorama branch 7.54 -> 6.54 ms, single-GPU step unchanged (37.3 -> 37.4 steps/s). The K partition depends on the
+# Split-K (pf_gemm_splitk_plan: only skinny deep-K problems — output tiles for at most half the SMs, >= 64 K-slabs, i.e. the 8x8 / 16x16-level
+# convolutions of a small batch, which otherwise stream their weights through a handful of SMs). The K partition depends on the
 # problem's M, so a sharded rank and the single-GPU run round a few convolutions differently (fp32 summation order):
 # PF_SPLIT_K=0 (or ops.SPLIT_K = False) restores the bit-identical sharded == unsharded behaviour the tests check.
 SPLIT_K = __import__("os").environ.get("PF_SPLIT_K", "1") != "0"
@@ -83,7 +82,7 @@ def gemm_taps(A: Tensor, B: Tensor, out: Tensor, *, M: int, Kc: int, taps: Seque
         block_n = 0
     elif not block_n and act != PF_ACT_GEGLU:
         block_n = _TUNED.get((int(M), B.shape[0], int(Kc), len(taps), int(image_map is not None),
-                              int(residual is not None)), 0)  # tile width | schedule << 16
+                              int(residual is not None)), 0)  # tile width
     a.block_n = int(block_n)
     if GEMM_LOG is not None:
         GEMM_LOG.append((int(M), B.shape[0], int(Kc), len(taps), int(act), image_map is not None,
@@ -118,7 +117,7 @@ def gemm_taps(A: Tensor, B: Tensor, out: Tensor, *, M: int, Kc: int, taps: Seque
     if k_splits is None:
         k_splits = _lib.lib().pf_gemm_splitk_plan(C.byref(a)) if (SPLIT_K and not row_stats and ln is None) else 1
     if k_splits > 1:
-        a.block_n = 0  # split-K runs on the tile-per-CTA schedule with the widest tile (operand bytes per FLOP matter)
+        a.block_n = 0  # split-K runs with the heuristic's (widest) tile: operand bytes per FLOP matter
         ws = torch.empty(k_splits * int(M) * B.shape[0], dtype=torch.float32, device=A.device)
         a.k_splits, a.splitk_ws = int(k_splits), ws.data_ptr()
         _count(1)

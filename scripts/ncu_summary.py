@@ -13,6 +13,7 @@ WANT = ["Kernel Name", "Block Size", "Grid Size", "gpu__time_duration.sum", "dra
         "launch__occupancy_limit_registers", "launch__occupancy_limit_shared_mem"]
 rows = list(csv.reader(sys.stdin))
 hdr, units, vals = rows[0], rows[1], rows[2]
+(Path(__file__).resolve().parent.parent / "profiles").mkdir(exist_ok=True)
 out = open(Path(__file__).resolve().parent.parent / "profiles" / f"{sys.argv[1]}_summary.txt", "w")
 for h, u, v in zip(hdr, units, vals):
     if h in WANT:

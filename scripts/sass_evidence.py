@@ -1,6 +1,6 @@
-"""Count the Blackwell-specific SASS mnemonics per kernel of libpanfusion_b200.so (cuobjdump, no GPU needed):
-tcgen05.mma -> UTC*MMA, tcgen05.ld/st -> LDTM/STTM, tcgen05.alloc -> UTCATOMSWS..., TMA -> UTMALDG/UTMASTG/UBLKCP.
-Usage: python scripts/sass_evidence.py > profiles/sass_evidence_r01.txt"""
+"""Count the Hopper-specific SASS mnemonics per kernel of libpanfusion_b200.so (cuobjdump, no GPU needed):
+wgmma.mma_async -> HGMMA, wgmma.fence / commit / wait -> WARPGROUP.*, TMA -> UTMALDG/UTMASTG/UBLKCP, mbarrier -> SYNCS.
+Usage: python scripts/sass_evidence.py"""
 import collections
 import re
 import subprocess
@@ -8,8 +8,8 @@ import sys
 from pathlib import Path
 
 LIB = Path(__file__).resolve().parent.parent / "panfusion_b200" / "lib" / "libpanfusion_b200.so"
-PAT = re.compile(r"\b(UTC[A-Z]*MMA[A-Z0-9_.]*|LDTM[A-Z0-9_.]*|STTM[A-Z0-9_.]*|UTMALDG[A-Z0-9_.]*|UTMASTG[A-Z0-9_.]*|UBLKCP[A-Z0-9_.]*|"
-                 r"UTCBAR[A-Z0-9_.]*|UTCATOMSWS[A-Z0-9_.]*|SYNCS[A-Z0-9_.]*|UTMAPF[A-Z0-9_.]*|UTMACMDFLUSH[A-Z0-9_.]*|MUFU\.EX2[A-Z0-9_.]*)")
+PAT = re.compile(r"\b(HGMMA[A-Z0-9_.]*|WARPGROUP[A-Z0-9_.]*|UTMALDG[A-Z0-9_.]*|UTMASTG[A-Z0-9_.]*|UBLKCP[A-Z0-9_.]*|"
+                 r"SYNCS[A-Z0-9_.]*|UTMAPF[A-Z0-9_.]*|UTMACMDFLUSH[A-Z0-9_.]*|MUFU\.EX2[A-Z0-9_.]*)")
 out = subprocess.run(["cuobjdump", "-sass", str(LIB)], capture_output=True, text=True, check=True).stdout
 kernels, cur = collections.OrderedDict(), None
 for line in out.splitlines():
@@ -21,7 +21,7 @@ for line in out.splitlines():
     if cur:
         for op in PAT.findall(line):
             kernels[cur][op.split(".")[0] if not op.startswith("MUFU") else "MUFU.EX2"] += 1
-print(f"# SASS evidence for {LIB.name} (sm_100a): Blackwell tensor-core / TMEM / TMA mnemonics per kernel")
+print(f"# SASS evidence for {LIB.name} (sm_90a): Hopper tensor-core / TMA mnemonics per kernel")
 for k, c in kernels.items():
-    if any(n.startswith(("UTC", "LDTM", "UTMA", "UBLKCP")) for n in c):
+    if any(n.startswith(("HGMMA", "UTMA", "UBLKCP")) for n in c):
         print(f"{k}\n    " + ", ".join(f"{n}={v}" for n, v in sorted(c.items())))

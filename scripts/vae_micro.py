@@ -1,4 +1,4 @@
-"""Time the image-space tail (SURVEY.md §8f rank 1) at BASELINE size on one B200: decode_latent of 8 view latents
+"""Time the image-space tail (SURVEY.md §8f rank 1) at BASELINE size on one GPU: decode_latent of 8 view latents
 64x64 + the circularly padded panorama decode (64x144 -> 512x1024) + tensor_to_image, SD-2 VAE decoder widths,
 random-init weights. Algorithmic FLOPs: 2.513 TFLOP per 512x512 image (hand count, 2*MAC) => 8 views 20.1 + pano
 (512x1152) 5.65 = 25.8 TFLOP. Usage: python scripts/vae_micro.py [--dtype bf16|fp16]"""

@@ -1,4 +1,4 @@
-"""-m gpu: tcgen05 flash attention (pf_fmha_fwd) against plain PyTorch fp32 softmax(q k^T s + bias) v on the same
+"""-m gpu: wgmma flash attention (pf_fmha_fwd) against plain PyTorch fp32 softmax(q k^T s + bias) v on the same
 16-bit-rounded inputs. The kernel rounds P to the 16-bit type before P V (like every flash kernel), so the
 tolerance is one 16-bit ulp of the output scale: fp16 rtol 1e-3 / atol 1e-3; bf16 rtol 8e-3 / atol 8e-3.
 """

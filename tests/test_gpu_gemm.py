@@ -1,4 +1,4 @@
-"""-m gpu: tcgen05 tap-GEMM (pf_gemm_taps) against a plain PyTorch fp32 reference of the same contraction.
+"""-m gpu: wgmma tap-GEMM (pf_gemm_taps) against a plain PyTorch fp32 reference of the same contraction.
 
 Inputs are rounded to the 16-bit compute type first, so the only differences are fp32 accumulation order and the
 final rounding of the output: tolerance rtol 1e-3 / atol 1e-4 for fp32 outputs (north_star), and one output ulp
@@ -53,6 +53,26 @@ def test_linear_epilogue(cuda_device, act, res_dtype):
     ops.gemm_taps(A, B, out, M=M, Kc=K, bias=bias, rowbias=rowbias, rows_per_group=rpg, residual=res,
                   act={"none": ops.PF_ACT_NONE, "silu": ops.PF_ACT_SILU, "gelu": ops.PF_ACT_GELU}[act])
     torch.testing.assert_close(out, ref, rtol=1e-3, atol=2e-4)
+
+
+@pytest.mark.parametrize("bn", [64, 128, 160])
+def test_linear_staged_epilogue(cuda_device, bn):
+    """16-bit output through the TMA-store epilogue at every tile width it serves: bias, per-group row bias, SiLU and a
+    16-bit residual that is TMA-prefetched into the staging tile (bn = 64 runs the deepest operand ring)."""
+    from panfusion_b200 import ops
+    M, N, K = 777, 640, 320
+    g = torch.Generator(device="cpu").manual_seed(11)
+    A = torch.randn(M, K, generator=g).bfloat16().to(cuda_device)
+    B = (torch.randn(N, K, generator=g) / K ** 0.5).bfloat16().to(cuda_device)
+    bias = torch.randn(N, generator=g).to(cuda_device)
+    rowbias = torch.randn(4, N, generator=g).to(cuda_device)
+    rpg = 200
+    res = torch.randn(M, N, generator=g).bfloat16().to(cuda_device)
+    ref = F.silu(A.float() @ B.float().T + bias + rowbias[(torch.arange(M, device=cuda_device) // rpg)]) + res.float()
+    out = torch.empty(M, N, dtype=torch.bfloat16, device=cuda_device)
+    ops.gemm_taps(A, B, out, M=M, Kc=K, bias=bias, rowbias=rowbias, rows_per_group=rpg, residual=res,
+                  act=ops.PF_ACT_SILU, block_n=bn)
+    torch.testing.assert_close(out.float(), ref, **_tol(torch.bfloat16))
 
 
 @pytest.mark.parametrize("N2,bn", [(2560, 160), (1280, 128), (5120, 0)])

@@ -7,7 +7,7 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
-# measured on B200: fp16 2.5e-3 / 2.5e-4, bf16 2.3e-2 / 2.0e-3 (SD-2 size, 23 layers)
+# measured on an H100: fp16 2.5e-3 / 2.4e-4, bf16 2.1e-2 / 2.0e-3 (SD-2 size, 23 layers)
 LIMITS = {torch.float16: (5e-3, 5e-4), torch.bfloat16: (4.7e-2, 4e-3)}
 
 

@@ -70,7 +70,7 @@ def test_training_loss_vs_oracle(cuda_device, dtype):
     out = step.loss(dev(latents), dev(pano_latent), dev(inp["prompt_embd"]), dev(inp["pano_prompt_embd"]), cams, t=dev(t),
                     noise=noise, pano_noise=dev(pano_noise))
     torch.cuda.synchronize()
-    # measured on B200: |loss - oracle| = 3.0e-5 (fp16), 1.1e-4 (bf16) on losses of 1.1 / 1.1 / 2.2 -> gates at ~3x
+    # measured on an H100: |loss - oracle| <= 5.5e-5 (fp16 and bf16) on losses of 1.1 / 1.1 / 2.2
     lim = {torch.float16: 1e-4, torch.bfloat16: 3e-4}[dtype]
     for k in ("loss_pers", "loss_pano", "loss"):
         got, want = out[k].item(), ref[k].item()
