@@ -341,6 +341,39 @@ int pf_eppa_pe(const double* cams_e2p, int V, int ph, int pw, int eh, int ew, co
                float* pers_pe, float* equi_pe, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * MVDiffusion correspondence-aware attention CPAttn (external/MVDiffusion/pano/modules.py:22-86,
+ * pano/utils.py:7-123): each pixel of view i attends to the 3x3 window around its homography correspondence in
+ * views (i-1) mod m and (i+1) mod m — 18 keys per query, key slot s = n*9 + (di+1)*3 + (dj+1) (n = 0: view i-1,
+ * n = 1: view i+1; di offsets x, dj offsets y).
+ * pf_cpattn_tables: homo_l / homo_r fp32 [G][m][2][9] row-major (per camera group, view i, neighbour n):
+ *   homo_l = K_n R_n^-1 R_i K_i^-1 (correspondences, utils.py:26-27), homo_r = K_i R_i^-1 R_n K_n^-1
+ *   (back-projection, modules.py:57-58). Query pixel (y, x) of the h x h level sits at image pixel
+ *   (s/2 + s x, s/2 + s y), s = img_size / h. Writes, per (g, i, query pixel, slot):
+ *   pos fp32 [G*m*h*w*18][4] = (grid_sample x, y in the neighbour's pixel units, xy_rel x, y) and
+ *   mask uint8 [G*m*h*w*18] (window position strictly inside the image, utils.py:74-75).
+ * pf_cpattn_gather: x = tokens [B*m*h*w, ldx] 16-bit (batch element b uses camera group b when G == B, group 0
+ *   when G == 1) -> keys [B*m*h*w*18, C] 16-bit = (bilinear sample + PosEmbedding(xy_rel)) * mask with
+ *   freq_bands[C/4] (transformer.py:169-209), and stats fp32 [B*m*h*w*18][2][2] = per-row (sum, sum of squares)
+ *   in slot 0 and zeros in slot 1: the ln_stats operand of pf_gemm_args (norm1 folded into the K|V GEMM).
+ * pf_cpattn_attn: q [ntok, ldq], kv [ntok*18, ldkv] = K in columns [0, C) and V in [C, 2C), out [ntok, ldo];
+ *   heads of width 32, softmax over the 18 keys in fp32 (masked keys included, like the reference).
+ * ------------------------------------------------------------------------------------------------ */
+int pf_cpattn_tables(const float* homo_l, const float* homo_r, int G, int m, int h, int w, int img_size, float* pos,
+                     uint8_t* mask, void* stream);
+int pf_cpattn_gather(const void* x, int ldx, int dtype, int B, int m, int h, int w, int C, int G, const float* pos,
+                     const uint8_t* mask, const float* freq_bands, void* keys, float* stats, void* stream);
+int pf_cpattn_attn(const void* q, int ldq, const void* kv, int ldkv, void* out, int ldo, int dtype, long long ntok,
+                   int C, float scale, void* stream);
+
+/* mp2e (external/Perspective_and_Equirectangular/mp2e.py as MvDiffusion.inference_and_save calls it, no mode):
+ * views uint8 [m, hp, wp, C] (C <= 4) -> out uint8 [He, We, C] = sum_v img_v w_v / sum_v w_v truncated, 255 where no
+ * view reaches; img_v / w_v are the view and its horizontal weight ramp warped by p2e's numpy path (cv2.remap with
+ * interpolation None = nearest, map rounded half to even, BORDER_WRAP) times the frustum mask. cams_p2e: m p2e camera
+ * records (PF_CAM_DOUBLES each, device). */
+int pf_mp2e(const uint8_t* views, int m, int hp, int wp, int C, const double* cams_p2e, int He, int We, uint8_t* out,
+            void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * View-sharded step (SURVEY.md 8e): device-initiated all-gather over NVLink peer mappings, capturable in a CUDA graph.
  * The reference has no model parallelism (Lightning DDP over prompts, main.py:63); this is the exchange the view partition
  * needs: models/pano/modules.py:44-48 lets every panorama query attend to the keys / values of ALL views, so each rank

@@ -86,7 +86,7 @@ EXPORTS = [
     "pf_fmha_fwd", "pf_bias_tile_flags", "pf_bias_tile_scan", "pf_bias_tile_pack",
     "pf_groupnorm_ws_floats", "pf_groupnorm_stats", "pf_conv_prep", "pf_gn_prep_ws_floats", "pf_gn_prep", "pf_layernorm",
     "pf_conv_in", "pf_conv_out", "pf_copy2d", "pf_pad_pano", "pf_softmax_rows", "pf_tensor_to_image", "pf_timestep_embed", "pf_cfg_ddim_step", "pf_cfg_ddim_step_dev",
-    "pf_eppa_tables", "pf_eppa_pe",
+    "pf_eppa_tables", "pf_eppa_pe", "pf_cpattn_tables", "pf_cpattn_gather", "pf_cpattn_attn", "pf_mp2e",
     "pf_allgather_views", "pf_enable_peer_access", "pf_comm_alloc", "pf_comm_free", "pf_ipc_export", "pf_ipc_open",
     "pf_ipc_close", "pf_embed_tokens", "pf_add_noise", "pf_mse_loss_ws_floats", "pf_mse_loss", "pf_gaussian_sample",
 ]

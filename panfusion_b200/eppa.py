@@ -64,6 +64,38 @@ class _SphericalPE(nn.Module):  # transformer.py:165-183: only the frequency tab
         self.register_buffer("freq_bands", base ** torch.linspace(0, n_freqs - 1, n_freqs))
 
 
+def pack_block(t: _Block, dev, dt) -> dict:
+    """The weights of a _Block packed for the kernels (once per device/dtype)."""
+    a = t.attn1
+    bn = ops.pick_block_n(t.ff.net[0].proj.weight.shape[0], ops.PF_ACT_GEGLU)
+    wp, bp = pack_geglu(t.ff.net[0].proj.weight.detach(), t.ff.net[0].proj.bias.detach(), bn)
+    return dict(
+        key=(dev, dt),
+        qkv=_Lin(torch.cat([a.to_q.weight, a.to_k.weight, a.to_v.weight], 0), None, dev, dt),
+        out=_Lin(a.to_out.weight, a.to_out.bias, dev, dt),
+        ff1_w=wp.to(dev, dt).contiguous(), ff1_b=bp.to(dev), ff1_bn=bn,
+        ff2=_Lin(t.ff.net[2].weight, t.ff.net[2].bias, dev, dt),
+        ff1_ln=_LinLN(t.ff.net[0].proj.weight, t.ff.net[0].proj.bias, t.norm2, dev, dt, geglu_bn=bn),
+        ln1=_Norm(t.norm1, dev), ln2=_Norm(t.norm2, dev), heads=a.heads)
+
+
+def block_tail(w: dict, o: Tensor, x_tok: Tensor, rows: int) -> Tensor:
+    """to_out(o) + x, then x + FF(norm2(x)) (transformer.py:159-160) on [rows, C] tokens; w = pack_block(...)."""
+    C = w["out"].n
+    new = lambda r, n: torch.empty((r, n), dtype=x_tok.dtype, device=x_tok.device)
+    if engine.FUSE_LN:  # norm2 folded into the GEGLU projection (engine._LinLN)
+        x1, st = ops.gemm_taps(o, w["out"].w, new(rows, C), M=rows, Kc=C, bias=w["out"].b, residual=x_tok,
+                               row_stats=True)
+        f = ops.gemm_taps(x1, w["ff1_ln"].w, new(rows, 4 * C), M=rows, Kc=C, bias=w["ff1_ln"].b,
+                          act=ops.PF_ACT_GEGLU, block_n=w["ff1_bn"], ln=(st, w["ff1_ln"].colsum, w["ff1_ln"].eps))
+        return ops.gemm_taps(f, w["ff2"].w, new(rows, C), M=rows, Kc=4 * C, bias=w["ff2"].b, residual=x1)
+    x1 = ops.gemm_taps(o, w["out"].w, new(rows, C), M=rows, Kc=C, bias=w["out"].b, residual=x_tok)
+    n2 = ops.layernorm(x1, w["ln2"].g, w["ln2"].b, w["ln2"].eps)
+    f = ops.gemm_taps(n2, w["ff1_w"], new(rows, 4 * C), M=rows, Kc=C, bias=w["ff1_b"], act=ops.PF_ACT_GEGLU,
+                      block_n=w["ff1_bn"])
+    return ops.gemm_taps(f, w["ff2"].w, new(rows, C), M=rows, Kc=4 * C, bias=w["ff2"].b, residual=x1)
+
+
 # resident form of the correspondence bias: tile-packed (only non-constant 128 x 64 tiles) unless PF_EPPA_DENSE_BIAS=1
 PACK_BIAS = __import__("os").environ.get("PF_EPPA_DENSE_BIAS", "0") == "0"
 
@@ -216,20 +248,8 @@ class WarpAttn(nn.Module):
 
     # ---- weight packing (once per device/dtype) --------------------------------------------------
     def _pack(self, dev, dt):
-        if self._packed is not None and self._packed["key"] == (dev, dt):
-            return self._packed
-        t = self.transformer
-        a = t.attn1
-        bn = ops.pick_block_n(t.ff.net[0].proj.weight.shape[0], ops.PF_ACT_GEGLU)
-        wp, bp = pack_geglu(t.ff.net[0].proj.weight.detach(), t.ff.net[0].proj.bias.detach(), bn)
-        self._packed = dict(
-            key=(dev, dt),
-            qkv=_Lin(torch.cat([a.to_q.weight, a.to_k.weight, a.to_v.weight], 0), None, dev, dt),
-            out=_Lin(a.to_out.weight, a.to_out.bias, dev, dt),
-            ff1_w=wp.to(dev, dt).contiguous(), ff1_b=bp.to(dev), ff1_bn=bn,
-            ff2=_Lin(t.ff.net[2].weight, t.ff.net[2].bias, dev, dt),
-            ff1_ln=_LinLN(t.ff.net[0].proj.weight, t.ff.net[0].proj.bias, t.norm2, dev, dt, geglu_bn=bn),
-            ln1=_Norm(t.norm1, dev), ln2=_Norm(t.norm2, dev), heads=a.heads)
+        if self._packed is None or self._packed["key"] != (dev, dt):
+            self._packed = pack_block(self.transformer, dev, dt)
         return self._packed
 
     def invalidate(self):
@@ -289,19 +309,7 @@ class WarpAttn(nn.Module):
         else:
             k_all, v_all = qkv_p[..., C:2 * C], qkv_p[..., 2 * C:]
 
-        def finish(o, x_tok, rows):
-            # to_out + residual, then x + FF(norm2(x)) (transformer.py:159-160)
-            if engine.FUSE_LN:  # norm2 folded into the GEGLU projection (engine._LinLN)
-                x1, st = ops.gemm_taps(o, w["out"].w, new(rows, C), M=rows, Kc=C, bias=w["out"].b, residual=x_tok,
-                                       row_stats=True)
-                f = ops.gemm_taps(x1, w["ff1_ln"].w, new(rows, 4 * C), M=rows, Kc=C, bias=w["ff1_ln"].b,
-                                  act=ops.PF_ACT_GEGLU, block_n=w["ff1_bn"], ln=(st, w["ff1_ln"].colsum, w["ff1_ln"].eps))
-                return ops.gemm_taps(f, w["ff2"].w, new(rows, C), M=rows, Kc=4 * C, bias=w["ff2"].b, residual=x1)
-            x1 = ops.gemm_taps(o, w["out"].w, new(rows, C), M=rows, Kc=C, bias=w["out"].b, residual=x_tok)
-            n2 = ops.layernorm(x1, w["ln2"].g, w["ln2"].b, w["ln2"].eps)
-            f = ops.gemm_taps(n2, w["ff1_w"], new(rows, 4 * C), M=rows, Kc=C, bias=w["ff1_b"], act=ops.PF_ACT_GEGLU,
-                              block_n=w["ff1_bn"])
-            return ops.gemm_taps(f, w["ff2"].w, new(rows, C), M=rows, Kc=4 * C, bias=w["ff2"].b, residual=x1)
+        finish = lambda o, x_tok, rows: block_tail(w, o, x_tok, rows)
 
         # The two directions only share their inputs: direction 1 (few pano tokens, under-filled launches) runs on the
         # panorama branch's side stream, concurrently with direction 2 on the caller's stream. Its result is consumed

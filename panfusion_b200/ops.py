@@ -468,3 +468,67 @@ def eppa_pe(cams_e2p: Tensor, ph: int, pw: int, eh: int, ew: int, freq_bands: Te
     _count(1)
     _lib.check(_lib.lib().pf_eppa_pe(_vp(cams_e2p), V, ph, pw, eh, ew, _vp(fb), nf, _vp(pers_pe), _vp(equi_pe), _st()))
     return pers_pe, equi_pe
+
+
+# ------------------------------------------------------------------------------------------------
+# MVDiffusion CPAttn
+# ------------------------------------------------------------------------------------------------
+CP_SLOTS = 18
+
+
+def cpattn_tables(homo_l: Tensor, homo_r: Tensor, h: int, w: int, img_size: int):
+    """homo_l / homo_r fp32 [G, m, 2, 3, 3] on the device -> (pos fp32 [G, m, h*w, 18, 4], mask uint8 [G, m, h*w, 18])."""
+    _lib.require_cuda(homo_l, homo_r)
+    assert homo_l.dtype == homo_r.dtype == torch.float32 and homo_l.is_contiguous() and homo_r.is_contiguous()
+    assert homo_l.shape == homo_r.shape and homo_l.dim() == 5 and tuple(homo_l.shape[2:]) == (2, 3, 3)
+    G, m = homo_l.shape[:2]
+    pos = torch.empty((G, m, h * w, CP_SLOTS, 4), dtype=torch.float32, device=homo_l.device)
+    mask = torch.empty((G, m, h * w, CP_SLOTS), dtype=torch.uint8, device=homo_l.device)
+    _count(1)
+    _lib.check(_lib.lib().pf_cpattn_tables(_vp(homo_l), _vp(homo_r), G, m, h, w, img_size, _vp(pos), _vp(mask), _st()))
+    return pos, mask
+
+
+def cpattn_gather(x: Tensor, B: int, m: int, h: int, w: int, pos: Tensor, mask: Tensor, freq_bands: Tensor):
+    """x tokens [B*m*h*w, >=C] 16-bit -> (keys [B*m*h*w*18, C] 16-bit, stats fp32 [B*m*h*w*18, 2, 2]) (pf_cpattn_gather)."""
+    _lib.require_cuda(x, pos, mask, freq_bands)
+    C = 4 * freq_bands.numel()
+    assert x.dim() == 2 and x.stride(1) == 1 and x.shape[0] == B * m * h * w and x.shape[1] >= C
+    assert pos.dtype == torch.float32 and pos.is_contiguous() and mask.dtype == torch.uint8 and mask.is_contiguous()
+    assert freq_bands.dtype == torch.float32 and freq_bands.is_contiguous()
+    G = pos.shape[0]
+    assert tuple(pos.shape) == (G, m, h * w, CP_SLOTS, 4) and tuple(mask.shape) == (G, m, h * w, CP_SLOTS)
+    rows = B * m * h * w * CP_SLOTS
+    keys = torch.empty((rows, C), dtype=x.dtype, device=x.device)
+    stats = torch.empty((rows, 2, 2), dtype=torch.float32, device=x.device)
+    _count(1)
+    _lib.check(_lib.lib().pf_cpattn_gather(_vp(x), x.stride(0), _lib.dtype_code(x.dtype), B, m, h, w, C, G, _vp(pos),
+                                           _vp(mask), _vp(freq_bands), _vp(keys), _vp(stats), _st()))
+    return keys, stats
+
+
+def cpattn_attn(q: Tensor, kv: Tensor, out: Tensor, scale: float) -> Tensor:
+    """q [T, >=C], kv [T*18, >=2C] (K | V), out [T, >=C], all 16-bit, last stride 1; heads of width 32 (pf_cpattn_attn)."""
+    _lib.require_cuda(q, kv, out)
+    ntok, ch = out.shape
+    assert q.stride(1) == kv.stride(1) == out.stride(1) == 1 and q.shape[0] == ntok and kv.shape[0] == ntok * CP_SLOTS
+    assert q.dtype == kv.dtype == out.dtype
+    _count(1)
+    _lib.check(_lib.lib().pf_cpattn_attn(_vp(q), q.stride(0), _vp(kv), kv.stride(0), _vp(out), out.stride(0),
+                                         _lib.dtype_code(q.dtype), C.c_longlong(ntok), ch, _f(scale), _st()))
+    return out
+
+
+def mp2e(views: Tensor, fov_deg, theta_deg, phi_deg, out_hw) -> Tensor:
+    """Stitch m uint8 views [m, hp, wp, C] (device) into one uint8 panorama [H, W, C] (pf_mp2e, mp2e.py:6-30)."""
+    from . import geometry
+    _lib.require_cuda(views)
+    assert views.dtype == torch.uint8 and views.dim() == 4 and views.is_contiguous()
+    m, hp, wp, ch = views.shape
+    cams, _ = geometry.camera_records("p2e", list(map(float, fov_deg)), list(map(float, theta_deg)),
+                                      list(map(float, phi_deg)), m, hp, wp, views.device)
+    H, W = (int(v) for v in out_hw)
+    out = torch.empty((H, W, ch), dtype=torch.uint8, device=views.device)
+    _count(1)
+    _lib.check(_lib.lib().pf_mp2e(_vp(views), m, hp, wp, ch, _vp(cams), H, W, _vp(out), _st()))
+    return out

@@ -63,6 +63,8 @@ def init_noise(bs, equi_h, equi_w, pers_h, pers_w, cameras, device, generator=No
 
 
 class PanFusionSampler:
+    _state_keys = ("latents", "pano")  # the static buffers a step updates in place (restored after a warm-up step)
+
     def __init__(self, mv_base_model, guidance_scale: float = 9.0, diff_timestep: int = 50, rot_diff: float = 90.0,
                  use_cuda_graph: bool = True):
         self.mv_base_model = mv_base_model
@@ -244,6 +246,21 @@ class PanFusionSampler:
         pano_img = pv.tensor_to_image(pv.decode_pano(pano, vae, latent_pad))
         return images, pano_img
 
+    def _graph_key(self, st, cameras) -> tuple:
+        """What a captured step depends on besides the contents of its static buffers."""
+        return (tuple(cameras["theta"].reshape(-1).tolist()), tuple(cameras["phi"].reshape(-1).tolist()),
+                tuple(cameras["FoV"].reshape(-1).tolist()), tuple(st["latents"].shape), tuple(st["pano"].shape),
+                st["latents"].data_ptr(), st["pano"].data_ptr(), st["prompt"].data_ptr(),
+                st["pano_cond"].data_ptr() if "pano_cond" in st else 0)
+
+    def _graph_tables(self, cameras) -> list:
+        """The cached camera tables a captured step reads by address."""
+        tables = getattr(getattr(self.mv_base_model, "cp_blocks_mid", None), "tables", None)
+        if tables is None:
+            return []
+        cam2 = {k: torch.cat([v] * 2).flatten(0, 1) for k, v in cameras.items()}
+        return tables.tensors_of(tables.camera_key(cam2))
+
     def _run_step(self, st, cameras):
         par = getattr(self.mv_base_model, "_par", None)
         self._steps_run = getattr(self, "_steps_run", 0) + 1
@@ -253,16 +270,13 @@ class PanFusionSampler:
             self._step_body(st, cameras)
             self.launches_per_step = ops.LAUNCHES - l0
             return
-        key = (tuple(cameras["theta"].reshape(-1).tolist()), tuple(cameras["phi"].reshape(-1).tolist()),
-               tuple(cameras["FoV"].reshape(-1).tolist()), tuple(st["latents"].shape), tuple(st["pano"].shape),
-               st["latents"].data_ptr(), st["pano"].data_ptr(), st["prompt"].data_ptr(),
-               st["pano_cond"].data_ptr() if "pano_cond" in st else 0)
+        key = self._graph_key(st, cameras)
         if par is not None and not (self.rot_diff % 360):
             key += (self._steps_run % 2,)  # a single rotation phase: still alternate between two graphs / buffer sets
         entry = self._graphs.get(key)
         if entry is None:
             # eager warm-up builds the camera tables / packs weights / sets kernel attributes, then capture
-            snap = {k: st[k].clone() for k in ("latents", "pano")}
+            snap = {k: st[k].clone() for k in self._state_keys}
             self._slot_seq = getattr(self, "_slot_seq", 1) + 1
             self.mv_base_model.par_slot = self._slot_seq  # this graph's own all-gather receive buffers
             self._step_body(st, cameras)
@@ -271,8 +285,8 @@ class PanFusionSampler:
                 # every rank has CONSUMED what the warm-up step gathered before the same receive buffers are used again
                 import torch.distributed as dist
                 dist.barrier(group=par.group)
-            st["latents"].copy_(snap["latents"])
-            st["pano"].copy_(snap["pano"])
+            for k in self._state_keys:
+                st[k].copy_(snap[k])
             if self._pool is None:
                 self._pool = torch.cuda.graph_pool_handle()
             l0 = ops.LAUNCHES
@@ -292,14 +306,11 @@ class PanFusionSampler:
                     self._step_body(st, cameras)
             self.launches_per_step = ops.LAUNCHES - l0  # kernels of ours inside one replayed step
             # the graph reads the camera tables by address: it co-owns them (the table cache is LRU-bounded)
-            tables = getattr(getattr(self.mv_base_model, "cp_blocks_mid", None), "tables", None)
-            if tables is not None:
-                cam2 = {k: torch.cat([v] * 2).flatten(0, 1) for k, v in cameras.items()}
-                g._pf_tables = tables.tensors_of(tables.camera_key(cam2))
+            g._pf_tables = self._graph_tables(cameras)
             while len(self._graphs) >= self.max_graphs:
                 self._graphs.pop(next(iter(self._graphs)))
             self._graphs[key] = g
-            st["latents"].copy_(snap["latents"])
-            st["pano"].copy_(snap["pano"])
+            for k in self._state_keys:
+                st[k].copy_(snap[k])
             entry = g
         entry.replay()
