@@ -121,8 +121,8 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     float acc[NACC];
 #pragma unroll
     for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
-    int prev_s = -1;
-    for (int kb = kb_begin; kb < kb_end; ++kb) {
+    // issue one K-slab's MMAs as one commit group (every range holds at least one slab)
+    auto issue_slab = [&](int kb) {
       const int s = (kb - kb_begin) % STAGES;
       mbar_wait(&full_bar[s], ((kb - kb_begin) / STAGES) & 1);
       const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
@@ -135,10 +135,16 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         Wgmma<BLOCK_N, BF16>::ss(acc, adesc + 2 * k, bdesc + 2 * k, 1);
       wgmma_commit();
       fence_regs(acc);
+    };
+    // The first slab is issued before the loop, so the zeroing above never meets an in-flight MMA at the loop head.
+    // Without the peel ptxas sees the accumulators defined both by those moves and by MMAs still in flight, and
+    // serialises every wgmma (a full wait after each m64 x BLOCK_N x k16, warning C7515).
+    issue_slab(kb_begin);
+    for (int kb = kb_begin + 1; kb < kb_end; ++kb) {
+      issue_slab(kb);
       wgmma_wait<1>();  // the previous slab's MMAs have retired: its slot goes back to the producer
       fence_regs(acc);
-      if (prev_s >= 0 && (et & 127) == 0) mbar_arrive(&empty_bar[prev_s]);
-      prev_s = s;
+      if ((et & 127) == 0) mbar_arrive(&empty_bar[(kb - 1 - kb_begin) % STAGES]);
     }
     wgmma_wait<0>();
     fence_regs(acc);
