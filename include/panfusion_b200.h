@@ -226,24 +226,20 @@ int pf_conv_prep(const void* x, void* out, int dtype, int N, int H, int W, int C
                  const float* gamma, const float* beta, int groups, int act, int circ, int up, int phases, int halo,
                  void* stream);
 
-/* pf_groupnorm_stats + pf_conv_prep in ONE launch (same semantics, same reference call sites), optionally over the channel
- * concatenation of two tensors (torch.cat([hidden, skip], dim=1) at MVGenModel.py:223,231,246,254):
+/* pf_groupnorm_stats + pf_conv_prep (same semantics, same reference call sites), optionally over the channel concatenation
+ * of two tensors (torch.cat([hidden, skip], dim=1) at MVGenModel.py:223,231,246,254):
  *   x = cat(x1[N*H*W, C1], x2[N*H*W, C2]) (x2 may be NULL); if cat_out != NULL the raw concatenation [N*H*W, C1+C2] is also
  *   written (the ResnetBlock2D shortcut convolution reads it);
  *   statistics over the image circularly extended by circ_stats columns (duplicated columns count twice), applied with
  *   gamma / beta (+ SiLU) while building the conv_prep layout (circ, up, phases, halo as in pf_conv_prep).
- * The kernel holds a per-image barrier between the statistics and the apply phase (the source is re-read from L2), so its
- * grid is capped at one CTA of <= 512 threads per SM — two such launches (the two UNet branches' streams) are always co-resident.
- * schedule: 1 = that fused launch, 2 = two launches (statistics with one CTA per slab, then the apply pass: no barrier, many
- * more CTAs per image), 0 = default (two launches unless
- * PF_GN_FUSED_MIN_N says otherwise). Same bits either way.
- * ws: pf_gn_prep_ws_floats(N, groups) floats of scratch; sync: 3*N ints that are ZERO on entry (restored to zero by the
- * kernel; concurrent launches need distinct slots). The partition of every sum depends on H*W only, never on N: results are
- * bit-identical for any batch size. */
+ * Two launches: the statistics with one CTA per slab of each image, then the apply pass with up to 64 CTAs per image (the
+ * source is re-read from L2). ws: pf_gn_prep_ws_floats(N, groups) floats of scratch; counters: N ints that are ZERO on
+ * entry (restored to zero by the kernel; concurrent launches need distinct slots). The partition of every sum depends on
+ * H*W only, never on N: results are bit-identical for any batch size. */
 int pf_gn_prep_ws_floats(int N, int groups);
 int pf_gn_prep(const void* x1, int ld1, int C1, const void* x2, int ld2, int C2, void* cat_out, void* out, int dtype,
                int N, int H, int W, int groups, float eps, const float* gamma, const float* beta, int act,
-               int circ_stats, int circ, int up, int phases, int halo, int schedule, float* ws, int* sync, void* stream);
+               int circ_stats, int circ, int up, int phases, int halo, float* ws, int* counters, void* stream);
 
 /* out[t, :] = LayerNorm(x[t, :] + pe[t % pe_rows, :]) * gamma + beta (pe fp32, may be NULL);
  * models/modules/transformer.py:157-160 (EPPA norm1 on x + query_pe / context, norm2) and the diffusers
@@ -258,13 +254,7 @@ int pf_layernorm(const void* x, int ldx, void* out, int ldo, int dtype, int T, i
 int pf_conv_in(const float* x, const float* w, const float* bias, void* out, int dtype, int N, int Cin, int H, int W,
                int Cout, int circ, int act, void* stream);
 
-/* conv_out (MVGenModel.py:279-295) over the PREPARED tensor: xp = pf_conv_prep(conv_norm_out statistics of the
- * un-padded tensor as the reference does at :288, SiLU, circ, halo = 1) of shape [N, H+2, W+2*circ+2, C] 16-bit
- * -> NCHW fp32 [N, Cout<=4, H, W]; circ = 1 for the panorama (pad_pano(1) -> conv -> unpad_pano(1)). */
-int pf_conv_out(const void* xp, int dtype, const float* w, const float* bias, float* out, int N, int H, int W, int C,
-                int Cout, int circ, void* stream);
-
-/* strided 2-D copy of 16-bit rows (skip concatenation, torch.cat at MVGenModel.py:223,231,246,254) */
+/* strided 2-D copy of 16-bit rows; src and dst may be column slices of wider tensors */
 int pf_copy2d(const void* src, int src_ld, void* dst, int dst_ld, long long rows, int cols, void* stream);
 
 /* pad_pano (utils/pano.py:74-99): out[r, j] = x[r, (j - pad) mod W] for j in [0, W + 2*pad) — circular padding of the

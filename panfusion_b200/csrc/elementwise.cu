@@ -124,57 +124,10 @@ conv_in_kernel(const float* __restrict__ x, const float* __restrict__ w, const f
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// conv_out: 3x3 conv (C -> Cout<=4) over the PREPARED input (conv_norm_out + SiLU already applied by pf_conv_prep,
-// zero halo of 1, panorama circularly extended by `circ` columns) -> NCHW fp32 (MVGenModel.py:279-295).
-// One warp per output pixel, lanes stride over channel pairs; weights fp32 [Cout, C, 3, 3] re-laid in smem as
-// [tap][Cout][C]. Reading the prepared tensor avoids re-evaluating GroupNorm+SiLU for each of the 9 taps.
-// ------------------------------------------------------------------------------------------------
-constexpr int CONV_OUT_PIX_PER_BLOCK = 64;
-
-template <bool BF16>
-__global__ void __launch_bounds__(256)
-conv_out_kernel(const uint16_t* __restrict__ xp, const float* __restrict__ w, const float* __restrict__ bias,
-                float* __restrict__ out, int N, int H, int W, int C, int Cout, int circ) {
-  extern __shared__ float s_w[];  // [9][Cout][C]
-  const int n = blockIdx.y;
-  for (int i = threadIdx.x; i < 9 * Cout * C; i += blockDim.x) {
-    const int c = i % C, co = (i / C) % Cout, tap = i / (C * Cout);
-    s_w[i] = w[((size_t)co * C + c) * 9 + tap];
-  }
-  __syncthreads();
-  const int Hp = H + 2, Wp = W + 2 * circ + 2;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  for (int pi = warp; pi < CONV_OUT_PIX_PER_BLOCK; pi += (blockDim.x >> 5)) {
-    const int pix = blockIdx.x * CONV_OUT_PIX_PER_BLOCK + pi;
-    if (pix >= H * W) break;
-    const int yy = pix / W, xx = pix % W;
-    float acc[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int dy = 0; dy < 3; ++dy) {
-#pragma unroll
-      for (int dx = 0; dx < 3; ++dx) {
-        const uint16_t* xr = xp + (((size_t)n * Hp + yy + dy) * Wp + xx + circ + dx) * C;
-        const float* wt = s_w + (dy * 3 + dx) * Cout * C;
-        for (int c = lane * 2; c < C; c += 64) {
-          const float2 f = unpack2<BF16>(__ldg(reinterpret_cast<const uint32_t*>(xr + c)));
-          for (int co = 0; co < Cout; ++co) acc[co] = fmaf(f.x, wt[co * C + c], fmaf(f.y, wt[co * C + c + 1], acc[co]));
-        }
-      }
-    }
-    for (int co = 0; co < Cout; ++co) {
-      const float v = warp_sum(acc[co]);
-      if (lane == 0) out[(((size_t)n * Cout + co) * H + yy) * W + xx] = v + (bias ? bias[co] : 0.f);
-    }
-  }
-}
-
-// strided 2-D copy of 16-bit rows (skip concatenation: torch.cat at MVGenModel.py:223,231,246,254)
+// strided 2-D copy of 16-bit rows; src and dst may be column slices of wider tensors
 __global__ void __launch_bounds__(256)
 copy2d_kernel(const uint16_t* __restrict__ src, int src_ld, uint16_t* __restrict__ dst, int dst_ld, long long rows,
               int cols) {
-  pdl_launch_dependents();
-  pdl_wait();
   const int vecs = cols / 8;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= rows * vecs) return;
@@ -397,31 +350,6 @@ extern "C" int pf_conv_in(const float* x, const float* w, const float* bias, voi
   return PF_OK;
 }
 
-extern "C" int pf_conv_out(const void* xp, int dtype, const float* w, const float* bias, float* out, int N, int H, int W,
-                           int C, int Cout, int circ, void* stream) {
-  using namespace pf;
-  PF_CHECK_ARG(xp && w && out, "pf_conv_out: null pointer");
-  PF_CHECK_ARG(dtype == PF_BF16 || dtype == PF_F16, "pf_conv_out: 16-bit input dtype required");
-  PF_CHECK_ARG(N > 0 && N <= 65535 && H > 0 && W > 0 && C % 2 == 0 && Cout >= 1 && Cout <= 4 && circ >= 0,
-               "pf_conv_out: bad shape");
-  const size_t smem = (size_t)9 * Cout * C * sizeof(float);
-  PF_CHECK_ARG(smem <= 200 * 1024, "pf_conv_out: C=%d too large", C);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  dim3 grid((H * W + CONV_OUT_PIX_PER_BLOCK - 1) / CONV_OUT_PIX_PER_BLOCK, N);
-  int rc;
-  if (dtype == PF_BF16) {
-    auto k = conv_out_kernel<true>;
-    if ((rc = check_cuda(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "conv_out attr"))) return rc;
-    k<<<grid, 256, smem, st>>>(static_cast<const uint16_t*>(xp), w, bias, out, N, H, W, C, Cout, circ);
-  } else {
-    auto k = conv_out_kernel<false>;
-    if ((rc = check_cuda(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "conv_out attr"))) return rc;
-    k<<<grid, 256, smem, st>>>(static_cast<const uint16_t*>(xp), w, bias, out, N, H, W, C, Cout, circ);
-  }
-  PF_CHECK_LAUNCH("conv_out_kernel");
-  return PF_OK;
-}
-
 extern "C" int pf_copy2d(const void* src, int src_ld, void* dst, int dst_ld, long long rows, int cols, void* stream) {
   using namespace pf;
   PF_CHECK_ARG(src && dst, "pf_copy2d: null pointer");
@@ -429,8 +357,8 @@ extern "C" int pf_copy2d(const void* src, int src_ld, void* dst, int dst_ld, lon
                "pf_copy2d: bad shape rows=%lld cols=%d", rows, cols);
   PF_CHECK_ARG(((uintptr_t)src & 15) == 0 && ((uintptr_t)dst & 15) == 0, "pf_copy2d: pointers must be 16-byte aligned");
   const long long total = rows * (cols / 8);
-  launch_pdl(copy2d_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, static_cast<cudaStream_t>(stream),
-             static_cast<const uint16_t*>(src), src_ld, static_cast<uint16_t*>(dst), dst_ld, rows, cols);
+  copy2d_kernel<<<(unsigned)((total + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint16_t*>(src), src_ld, static_cast<uint16_t*>(dst), dst_ld, rows, cols);
   PF_CHECK_LAUNCH("copy2d_kernel");
   return PF_OK;
 }

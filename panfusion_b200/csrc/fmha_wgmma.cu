@@ -83,7 +83,6 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   uint64_t* kv_full = bars + 1;
   uint64_t* kv_empty = kv_full + STAGES;
 
-  pdl_launch_dependents();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int h = blockIdx.x % p.H;  // heads fastest: CTAs sharing a bias tile run together (L2 reuse)
   const int qt = blockIdx.x / p.H;
@@ -103,7 +102,6 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();  // Q/K/V (and the bias flags) written by the predecessor are visible from here on
 
   if (warp == 8) {
     if (lane == 0) {
@@ -318,7 +316,7 @@ static int launch_fmha(const pf_fmha_args* a, cudaStream_t st) {
     attr_set = true;
   }
   dim3 grid(((a->Lq + FA_BLOCK_M - 1) / FA_BLOCK_M) * a->H, a->B);
-  if ((rc = check_cuda(launch_pdl(kern, grid, dim3(FA_THREADS), SMEM, st, tmQ, tmK, tmV, p), "launch(fmha)"))) return rc;
+  kern<<<grid, FA_THREADS, SMEM, st>>>(tmQ, tmK, tmV, p);
   PF_CHECK_LAUNCH("fmha_fwd_kernel");
   return PF_OK;
 }

@@ -60,7 +60,6 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   float* s_bias = reinterpret_cast<float*>(staging + STAGING_BYTES + gemm_bar_bytes(STAGES));  // [BLOCK_N]
   float* s_cs = s_bias + BLOCK_N;                                            // [BLOCK_N] LayerNorm column sums
 
-  pdl_launch_dependents();  // the next kernel of the stream may start its prologue while this one runs
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int n_tiles = p.N / BLOCK_N;
@@ -84,7 +83,6 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();  // everything above touched only on-chip state; operands of the predecessor are visible from here on
 
   if (warp == 8) {
     // ------------------------------ TMA producer ------------------------------
@@ -506,8 +504,7 @@ static int launch_gemm(const pf_gemm_args* a, const GemmKernelParams& kp, cudaSt
     if (rc) return rc;
     attr_set[bf] = true;
   }
-  int rc = check_cuda(launch_pdl(kern, grid, dim3(GEMM_THREADS), SMEM, st, tmA, tmB, tmC, tmR, kp), "launch(gemm)");
-  if (rc) return rc;
+  kern<<<grid, GEMM_THREADS, SMEM, st>>>(tmA, tmB, tmC, tmR, kp);
   PF_CHECK_LAUNCH("gemm_taps_kernel");
   return PF_OK;
 }

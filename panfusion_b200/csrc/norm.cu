@@ -2,123 +2,19 @@
 //
 //  * pf_groupnorm_stats : GroupNorm statistics of a channels-last image, optionally over the circularly padded
 //    image (the reference normalises the W+2*circ wide tensor: models/pano/MVGenModel.py:110-115 wraps every
-//    panorama ResnetBlock2D in pad_pano(2)/unpad_pano(2), so columns {0,1,W-2,W-1} count twice).
+//    panorama ResnetBlock2D in pad_pano(2)/unpad_pano(2), so columns {0,1,W-2,W-1} count twice). It is the
+//    statistics launch of pf_gn_prep with its own partition of the image.
 //  * pf_conv_prep       : GroupNorm-apply (+SiLU) fused with building the tap-GEMM's A operand: circular column
 //    extension (utils/pano.py:74-105), nearest x2 upsampling (Upsample2D), zero halo, or the four stride-2
 //    phase images (Downsample2D). Replaces norm1/norm2 + nonlinearity of ResnetBlock2D, Transformer2DModel.norm,
 //    and ~60 pad_pano / unpad_pano copies per step.
+//  * pf_gn_prep         : pf_groupnorm_stats + pf_conv_prep as two launches of one kernel (statistics, then apply),
+//    optionally over the skip concatenation of two tensors.
 //  * pf_layernorm       : LayerNorm(x + pe) per token (models/modules/transformer.py:157-160, diffusers
 //    BasicTransformerBlock norm1/2/3).
 #include "pf_common.cuh"
 
 namespace pf {
-
-constexpr int GN_MAX_CHUNKS = 64;
-
-__device__ __forceinline__ int gn_chunks(int hw) {
-  int c = hw / 64;
-  return c < 1 ? 1 : (c > GN_MAX_CHUNKS ? GN_MAX_CHUNKS : c);
-}
-
-// partial sums: grid (chunks, N); thread <-> (8-channel vector, pixel lane)
-template <bool BF16>
-__global__ void __launch_bounds__(512)
-gn_partial_kernel(const uint16_t* __restrict__ x, int H, int W, int C, int ld, int groups, int circ,
-                  float* __restrict__ ws, int* __restrict__ counters, float count, float eps,
-                  float* __restrict__ mean_rstd) {
-  extern __shared__ float s_acc[];  // [ppi][2][C] per-pixel-lane partials (fixed-order reduction: deterministic)
-  pdl_launch_dependents();
-  pdl_wait();
-  const int vecs = C / 8;
-  const int ppi = blockDim.x / vecs;
-  const int v = threadIdx.x % vecs, pl = threadIdx.x / vecs;
-  const int n = blockIdx.y, chunks = gridDim.x;
-  const int hw = H * W;
-  const int per = (hw + chunks - 1) / chunks;
-  const int p_begin = blockIdx.x * per, p_end = min(hw, p_begin + per);
-  float s[8], q[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) s[e] = q[e] = 0.f;
-  {
-    const uint16_t* base = x + (size_t)n * hw * ld + v * 8;
-    auto accum = [&](const uint4& raw, int p) {
-      float wgt = 1.f;
-      if (circ > 0) {
-        const int col = p % W;
-        wgt += (col < circ ? 1.f : 0.f) + (col >= W - circ ? 1.f : 0.f);
-      }
-      const uint32_t w4[4] = {raw.x, raw.y, raw.z, raw.w};
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float2 f = unpack2<BF16>(w4[e]);
-        s[2 * e] += wgt * f.x;
-        q[2 * e] += wgt * f.x * f.x;
-        s[2 * e + 1] += wgt * f.y;
-        q[2 * e + 1] += wgt * f.y * f.y;
-      }
-    };
-    int p = p_begin + pl;
-    // four independent 16-byte loads in flight per thread
-    for (; p + 3 * ppi < p_end; p += 4 * ppi) {
-      const uint4 r0 = __ldg(reinterpret_cast<const uint4*>(base + (size_t)p * ld));
-      const uint4 r1 = __ldg(reinterpret_cast<const uint4*>(base + (size_t)(p + ppi) * ld));
-      const uint4 r2 = __ldg(reinterpret_cast<const uint4*>(base + (size_t)(p + 2 * ppi) * ld));
-      const uint4 r3 = __ldg(reinterpret_cast<const uint4*>(base + (size_t)(p + 3 * ppi) * ld));
-      accum(r0, p);
-      accum(r1, p + ppi);
-      accum(r2, p + 2 * ppi);
-      accum(r3, p + 3 * ppi);
-    }
-    for (; p < p_end; p += ppi) accum(__ldg(reinterpret_cast<const uint4*>(base + (size_t)p * ld)), p);
-    float* mine = s_acc + (size_t)pl * 2 * C;
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      mine[v * 8 + e] = s[e];
-      mine[C + v * 8 + e] = q[e];
-    }
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) {
-    float a = s_acc[i];
-    for (int l = 1; l < ppi; ++l) a += s_acc[(size_t)l * 2 * C + i];
-    s_acc[i] = a;
-  }
-  __syncthreads();
-  const int cpg = C / groups;
-  for (int g = threadIdx.x; g < groups; g += blockDim.x) {
-    float a = 0.f, b = 0.f;
-    for (int c = g * cpg; c < (g + 1) * cpg; ++c) {
-      a += s_acc[c];
-      b += s_acc[C + c];
-    }
-    float* o = ws + (((size_t)n * chunks + blockIdx.x) * groups + g) * 2;
-    o[0] = a;
-    o[1] = b;
-  }
-  // The last CTA of image n to arrive reduces the chunk partials in a FIXED order (deterministic) and publishes
-  // mean / rstd — no separate finalize launch. counters[n] returns to 0 for the next use.
-  __shared__ int s_last;
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) s_last = (atomicAdd(&counters[n], 1) == chunks - 1);
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
-  for (int g = threadIdx.x; g < groups; g += blockDim.x) {
-    double a = 0.0, b = 0.0;
-    for (int c = 0; c < chunks; ++c) {
-      const float* o = ws + (((size_t)n * chunks + c) * groups + g) * 2;
-      a += __ldcg(o);
-      b += __ldcg(o + 1);
-    }
-    const double mean = a / count;
-    double var = b / count - mean * mean;
-    if (var < 0.0) var = 0.0;
-    mean_rstd[((size_t)n * groups + g) * 2 + 0] = float(mean);
-    mean_rstd[((size_t)n * groups + g) * 2 + 1] = float(1.0 / sqrt(var + double(eps)));
-  }
-  if (threadIdx.x == 0) counters[n] = 0;
-}
 
 // ------------------------------------------------------------------------------------------------
 // conv_prep: thread <-> (output position, 8-channel vector)
@@ -138,8 +34,6 @@ struct PrepParams {
 // row's image is built once per CTA in shared memory and the inner loop is load -> 8 FMA (+SiLU) -> store.
 template <bool BF16>
 __global__ void __launch_bounds__(256) conv_prep_kernel(const PrepParams p) {
-  pdl_launch_dependents();
-  pdl_wait();  // the GroupNorm statistics staged below come from the predecessor
   extern __shared__ float s_ss[];  // [2][C] scale, shift
   const int vecs = p.C / 8;
   int rowid = blockIdx.y;
@@ -208,30 +102,20 @@ __global__ void __launch_bounds__(256) conv_prep_kernel(const PrepParams p) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// gn_prep: GroupNorm statistics + apply (+SiLU) + conv_prep layout in ONE launch (pf_gn_prep).
+// gn_prep: GroupNorm statistics, then GroupNorm-apply (+SiLU) + conv_prep layout (pf_gn_prep); the statistics launch
+// alone is pf_groupnorm_stats.
 //
-// grid = (chunks, G) with chunks * G <= the SM count, so that every CTA of the launch (and of one more such launch on
-// the other branch's stream) is co-resident: the kernel contains a per-image barrier. CTA (c, y) serves images
-// y, y + G, ... in turn. The statistics are accumulated per SLAB — a fixed partition of the image into `slabs` pixel
-// ranges that depends on the image size ONLY — and the slabs are summed in slab order; how many slabs a CTA owns (few
-// CTAs per image for a big batch, many for a small one) does not enter any floating-point sum, so the result is the same,
-// bit for bit, whatever the batch size (a view-sharded rank reproduces the single-GPU run). Phase 1: each CTA sums its band
-// of source pixels per channel (two sources = the skip concatenation torch.cat([hidden, skip], 1), optionally also
-// written out raw), publishes per-group partials, and the LAST CTA of the image to arrive reduces them in a fixed
-// order (deterministic) into mean / rstd and releases the image's flag. Phase 2: after acquiring the flag each CTA
-// produces its share of the image's output positions — the source pixels are re-read from L2, not HBM.
-// sync[3n .. 3n+2] = {arrivals, flag, departures}: all zero on entry and restored to zero by the last CTA to leave.
+// STATS launch, grid (slabs, N): CTA (s, n) sums slab s of image n per channel — the slabs are a fixed partition of the
+// image into pixel ranges that depends on the image size ONLY — and publishes per-group partials (two sources = the skip
+// concatenation torch.cat([hidden, skip], 1), optionally also written out raw). The LAST CTA of the image to arrive
+// reduces the partials in slab order into mean / rstd and re-arms counters[n]. No floating-point sum depends on the batch
+// size, so the result is the same, bit for bit, for any N (a view-sharded rank reproduces the single-GPU run).
+// APPLY launch, grid (ctas, N): CTA (c, n) produces its share of image n's output positions; the source pixels are
+// re-read from L2, not HBM.
 // ------------------------------------------------------------------------------------------------
-constexpr int GNP_MAX_SLABS = 64;  // upper bound of the statistics partition of one image (fixed by its size)
-
-__device__ __forceinline__ int ld_acquire_s32(const int* p) {
-  int v;
-  asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void st_release_s32(int* p, int v) {
-  asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
+constexpr int GN_MAX_SLABS = 64;   // upper bound of the statistics partition of one image (sizes the workspace)
+constexpr int GN_PREP_SLABS = 32;  // pf_gn_prep: at most 32 slabs per image
+constexpr int GN_APPLY_CTAS = 64;  // pf_gn_prep: at most 64 apply CTAs per image
 
 struct GnPrepParams {
   const uint16_t* x1;
@@ -240,41 +124,32 @@ struct GnPrepParams {
   uint16_t* out;
   const float* gamma;
   const float* beta;
-  float* ws;            // [N][slabs][groups][2] partials, then [N][groups][2] mean/rstd at ws_mr
+  float* ws;            // [N][slabs][groups][2] partials
+  float* mean_rstd;     // [N][groups][2]
+  int* counters;        // [N], zero on entry and on exit of the statistics launch
   int slabs;            // statistics partition of an image: a function of H*W only
-  float* ws_mr;
-  int* sync;            // [N][3]
   int N, H, W, C1, C2, ld1, ld2, groups, act, circ_stats, circ, up, phases, halo;
   int Ho, Wo;
   float count, eps;
 };
 
-// MODE 0: fused (statistics, per-image barrier, apply) — large batches. MODE 1: statistics only, one CTA per slab, the last
-// CTA of an image finalises mean / rstd. MODE 2: apply only (reads mean / rstd), any number of CTAs per image. 1 + 2 are two
-// launches without a barrier and with far more CTAs per image: faster for the small batches of a sharded rank. The
-// statistics code is shared, so all modes produce the same bits.
-template <bool BF16, int MODE>
+template <bool BF16, bool STATS>
 __global__ void __launch_bounds__(512, 2) gn_prep_kernel(const GnPrepParams p) {
-  extern __shared__ float s_acc[];  // phase 1: [ppi][2][C] partials; phase 2: [2][C] scale / shift
-  pdl_launch_dependents();
-  pdl_wait();
+  extern __shared__ float s_acc[];  // statistics: [ppi][2][C] partials; apply: [2][C] scale / shift
   const int C = p.C1 + p.C2;
   const int vecs = C / 8, vecs1 = p.C1 / 8;
-  const int ppi = blockDim.x / vecs;
+  const int ppi = blockDim.x / vecs;  // blockDim.x is a multiple of vecs
   const int v = threadIdx.x % vecs, pl = threadIdx.x / vecs;
-  const int chunks = gridDim.x;
+  const int n = blockIdx.y;
   const int hw = p.H * p.W;
   const bool second = v >= vecs1;
   const int ld = second ? p.ld2 : p.ld1;
-  const bool active = pl < ppi;     // blockDim.x is a multiple of vecs, so every thread is active; kept for clarity
-  __shared__ int s_last;
- for (int n = blockIdx.y; n < p.N; n += gridDim.y) {
   const uint16_t* src = second ? p.x2 + (size_t)n * hw * p.ld2 + (v - vecs1) * 8 : p.x1 + (size_t)n * hw * p.ld1 + v * 8;
-  // ---------------- phase 1: statistics, one slab at a time (this CTA owns slabs/chunks consecutive slabs) ----------------
   const int cpg = C / p.groups;
-  const int slabs_per_cta = MODE == 2 ? 0 : p.slabs / chunks;
-  const int per = (hw + p.slabs - 1) / p.slabs;
-  for (int sl = blockIdx.x * slabs_per_cta; sl < (blockIdx.x + 1) * slabs_per_cta; ++sl) {
+  float* mr = p.mean_rstd + (size_t)n * p.groups * 2;
+  if constexpr (STATS) {
+    const int sl = blockIdx.x;
+    const int per = (hw + p.slabs - 1) / p.slabs;
     const int p_begin = sl * per, p_end = min(hw, p_begin + per);
     float s[8], q[8];
 #pragma unroll
@@ -296,25 +171,24 @@ __global__ void __launch_bounds__(512, 2) gn_prep_kernel(const GnPrepParams p) {
       }
       if (p.cat_out) *reinterpret_cast<uint4*>(p.cat_out + ((size_t)n * hw + px) * C + v * 8) = raw;
     };
-    if (active) {
-      int px = p_begin + pl;
-      for (; px + 3 * ppi < p_end; px += 4 * ppi) {
-        const uint4 r0 = __ldg(reinterpret_cast<const uint4*>(src + (size_t)px * ld));
-        const uint4 r1 = __ldg(reinterpret_cast<const uint4*>(src + (size_t)(px + ppi) * ld));
-        const uint4 r2 = __ldg(reinterpret_cast<const uint4*>(src + (size_t)(px + 2 * ppi) * ld));
-        const uint4 r3 = __ldg(reinterpret_cast<const uint4*>(src + (size_t)(px + 3 * ppi) * ld));
-        accum(r0, px);
-        accum(r1, px + ppi);
-        accum(r2, px + 2 * ppi);
-        accum(r3, px + 3 * ppi);
-      }
-      for (; px < p_end; px += ppi) accum(__ldg(reinterpret_cast<const uint4*>(src + (size_t)px * ld)), px);
-      float* mine = s_acc + (size_t)pl * 2 * C;
+    int px = p_begin + pl;
+    // four independent 16-byte loads in flight per thread
+    for (; px + 3 * ppi < p_end; px += 4 * ppi) {
+      const uint4 r0 = __ldg(reinterpret_cast<const uint4*>(src + (size_t)px * ld));
+      const uint4 r1 = __ldg(reinterpret_cast<const uint4*>(src + (size_t)(px + ppi) * ld));
+      const uint4 r2 = __ldg(reinterpret_cast<const uint4*>(src + (size_t)(px + 2 * ppi) * ld));
+      const uint4 r3 = __ldg(reinterpret_cast<const uint4*>(src + (size_t)(px + 3 * ppi) * ld));
+      accum(r0, px);
+      accum(r1, px + ppi);
+      accum(r2, px + 2 * ppi);
+      accum(r3, px + 3 * ppi);
+    }
+    for (; px < p_end; px += ppi) accum(__ldg(reinterpret_cast<const uint4*>(src + (size_t)px * ld)), px);
+    float* mine = s_acc + (size_t)pl * 2 * C;
 #pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        mine[v * 8 + e] = s[e];
-        mine[C + v * 8 + e] = q[e];
-      }
+    for (int e = 0; e < 8; ++e) {
+      mine[v * 8 + e] = s[e];
+      mine[C + v * 8 + e] = q[e];
     }
     __syncthreads();
     for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) {
@@ -333,17 +207,12 @@ __global__ void __launch_bounds__(512, 2) gn_prep_kernel(const GnPrepParams p) {
       o[0] = a;
       o[1] = b;
     }
-    __syncthreads();  // s_acc is rewritten by the next slab
-  }
-  // ---------------- per-image barrier ----------------
-  int* sync = p.sync + 3 * n;
-  float* mr = p.ws_mr + (size_t)n * p.groups * 2;
-  if constexpr (MODE != 2) {
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) s_last = (atomicAdd(&sync[0], 1) == chunks - 1);
-  __syncthreads();
-  if (s_last) {
+    __shared__ int s_last;
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) s_last = (atomicAdd(&p.counters[n], 1) == p.slabs - 1);
+    __syncthreads();
+    if (!s_last) return;
     __threadfence();
     for (int g = threadIdx.x; g < p.groups; g += blockDim.x) {
       double a = 0.0, b = 0.0;
@@ -358,121 +227,92 @@ __global__ void __launch_bounds__(512, 2) gn_prep_kernel(const GnPrepParams p) {
       mr[g * 2 + 0] = float(mean);
       mr[g * 2 + 1] = float(1.0 / sqrt(var + double(p.eps)));
     }
-    __threadfence();
-    __syncthreads();
-    if constexpr (MODE == 1) {
-      if (threadIdx.x == 0) sync[0] = 0;  // re-armed for the next launch; the apply kernel is ordered by the stream
-    } else {
-      if (threadIdx.x == 0) st_release_s32(&sync[1], 1);
+    if (threadIdx.x == 0) p.counters[n] = 0;  // the next launch is ordered behind this one by the stream
+  } else {
+    // scale / shift of this image into shared memory
+    for (int c = threadIdx.x; c < C; c += blockDim.x) {
+      const int g = c / cpg;
+      const float mean = __ldcg(mr + g * 2), rstd = __ldcg(mr + g * 2 + 1);
+      const float sc = rstd * __ldg(p.gamma + c);
+      s_acc[c] = sc;
+      s_acc[C + c] = __ldg(p.beta + c) - mean * sc;
     }
-  } else if constexpr (MODE == 0) {
-    if (threadIdx.x == 0) {
-      unsigned spins = 0;
-      while (ld_acquire_s32(&sync[1]) == 0) {
-        __nanosleep(40);
-        if (++spins > (1u << 26)) {  // ~3 s: a lost CTA is a bug (grid larger than the co-resident capacity)
-          printf("pf gn_prep_kernel: image barrier timed out (block %d,%d)\n", blockIdx.x, blockIdx.y);
-          __trap();
+    __syncthreads();
+    const int We = p.W + 2 * p.circ;
+    const int Hu = p.H * p.up, Wu = We * p.up;
+    const int total = p.phases * p.Ho * p.Wo;
+    const int ctas = gridDim.x;
+    const int per_o = (total + ctas - 1) / ctas;
+    const int o_begin = blockIdx.x * per_o, o_end = min(total, o_begin + per_o);
+    const float4 s0 = *reinterpret_cast<const float4*>(s_acc + v * 8), s1 = *reinterpret_cast<const float4*>(s_acc + v * 8 + 4);
+    const float4 h0 = *reinterpret_cast<const float4*>(s_acc + C + v * 8), h1 = *reinterpret_cast<const float4*>(s_acc + C + v * 8 + 4);
+    const size_t img_out = (size_t)p.Ho * p.Wo;
+    const int hw_o = p.Ho * p.Wo;
+    // (output position) -> (source pixel offset or -1 for the zero halo, output vector pointer)
+    auto locate = [&](int o, long long& soff, uint4*& dst) {
+      const int ph = o / hw_o;
+      const int r = o - ph * hw_o;
+      const int i = r / p.Wo, j = r - i * p.Wo;
+      int yy, xx;
+      if (p.phases == 4) {
+        yy = 2 * i + (ph >> 1) - 1;
+        xx = 2 * j + (ph & 1) - 1;
+      } else {
+        yy = i - p.halo;
+        xx = j - p.halo;
+      }
+      soff = -1;
+      if (yy >= 0 && yy < Hu && xx >= 0 && xx < Wu) {
+        const int sy = yy / p.up;
+        int sx = xx / p.up - p.circ;
+        if (sx < 0) sx += p.W;
+        else if (sx >= p.W) sx -= p.W;
+        soff = ((long long)sy * p.W + sx) * ld;
+      }
+      dst = reinterpret_cast<uint4*>(p.out + (((size_t)ph * p.N + n) * img_out + r) * C + v * 8);  // [phases][N][Ho][Wo][C]
+    };
+    auto finish = [&](const uint4& raw, bool live, uint4* dst) {
+      uint4 outv = make_uint4(0, 0, 0, 0);
+      if (live) {
+        const uint32_t w4[4] = {raw.x, raw.y, raw.z, raw.w};
+        float f[8];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float2 t = unpack2<BF16>(w4[e]);
+          f[2 * e] = t.x;
+          f[2 * e + 1] = t.y;
         }
+        f[0] = fmaf(f[0], s0.x, h0.x); f[1] = fmaf(f[1], s0.y, h0.y); f[2] = fmaf(f[2], s0.z, h0.z); f[3] = fmaf(f[3], s0.w, h0.w);
+        f[4] = fmaf(f[4], s1.x, h1.x); f[5] = fmaf(f[5], s1.y, h1.y); f[6] = fmaf(f[6], s1.z, h1.z); f[7] = fmaf(f[7], s1.w, h1.w);
+        if (p.act == PF_ACT_SILU) {
+#pragma unroll
+          for (int e = 0; e < 8; ++e) f[e] = silu_f(f[e]);
+        }
+        outv = make_uint4(pack2<BF16>(f[0], f[1]), pack2<BF16>(f[2], f[3]), pack2<BF16>(f[4], f[5]), pack2<BF16>(f[6], f[7]));
       }
-    }
-    __syncthreads();
-  }
-  }
-  if constexpr (MODE == 1) continue;
-  // scale / shift of this image into shared memory (aliases the phase-1 partials)
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    const int g = c / cpg;
-    const float mean = __ldcg(mr + g * 2), rstd = __ldcg(mr + g * 2 + 1);
-    const float sc = rstd * __ldg(p.gamma + c);
-    s_acc[c] = sc;
-    s_acc[C + c] = __ldg(p.beta + c) - mean * sc;
-  }
-  __syncthreads();
-  // everyone has read mean / rstd: the last CTA to get here re-arms the image's barrier for the next launch
-  if (MODE == 0 && threadIdx.x == 0) {
-    if (atomicAdd(&sync[2], 1) == chunks - 1) {
-      sync[0] = 0;
-      sync[2] = 0;
-      st_release_s32(&sync[1], 0);
-    }
-  }
-  // ---------------- phase 2: this CTA's share of the image's output positions ----------------
-  const int We = p.W + 2 * p.circ;
-  const int Hu = p.H * p.up, Wu = We * p.up;
-  const int total = p.phases * p.Ho * p.Wo;
-  const int per_o = (total + chunks - 1) / chunks;
-  const int o_begin = blockIdx.x * per_o, o_end = min(total, o_begin + per_o);
-  const float4 s0 = *reinterpret_cast<const float4*>(s_acc + v * 8), s1 = *reinterpret_cast<const float4*>(s_acc + v * 8 + 4);
-  const float4 h0 = *reinterpret_cast<const float4*>(s_acc + C + v * 8), h1 = *reinterpret_cast<const float4*>(s_acc + C + v * 8 + 4);
-  const size_t img_out = (size_t)p.Ho * p.Wo;
-  const int hw_o = p.Ho * p.Wo;
-  // (output position) -> (source pixel offset or -1 for the zero halo, output vector pointer)
-  auto locate = [&](int o, long long& soff, uint4*& dst) {
-    const int ph = o / hw_o;
-    const int r = o - ph * hw_o;
-    const int i = r / p.Wo, j = r - i * p.Wo;
-    int yy, xx;
-    if (p.phases == 4) {
-      yy = 2 * i + (ph >> 1) - 1;
-      xx = 2 * j + (ph & 1) - 1;
-    } else {
-      yy = i - p.halo;
-      xx = j - p.halo;
-    }
-    soff = -1;
-    if (yy >= 0 && yy < Hu && xx >= 0 && xx < Wu) {
-      const int sy = yy / p.up;
-      int sx = xx / p.up - p.circ;
-      if (sx < 0) sx += p.W;
-      else if (sx >= p.W) sx -= p.W;
-      soff = ((long long)sy * p.W + sx) * ld;
-    }
-    dst = reinterpret_cast<uint4*>(p.out + (((size_t)ph * p.N + n) * img_out + r) * C + v * 8);  // [phases][N][Ho][Wo][C]
-  };
-  auto finish = [&](const uint4& raw, bool live, uint4* dst) {
-    uint4 outv = make_uint4(0, 0, 0, 0);
-    if (live) {
-      const uint32_t w4[4] = {raw.x, raw.y, raw.z, raw.w};
-      float f[8];
+      *dst = outv;
+    };
+    const uint4 z4 = make_uint4(0, 0, 0, 0);
+    int o = o_begin + pl;
+    for (; o + 3 * ppi < o_end; o += 4 * ppi) {  // four independent L2 loads in flight per thread
+      long long so[4];
+      uint4* dst[4];
+      uint4 raw[4];
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float2 t = unpack2<BF16>(w4[e]);
-        f[2 * e] = t.x;
-        f[2 * e + 1] = t.y;
-      }
-      f[0] = fmaf(f[0], s0.x, h0.x); f[1] = fmaf(f[1], s0.y, h0.y); f[2] = fmaf(f[2], s0.z, h0.z); f[3] = fmaf(f[3], s0.w, h0.w);
-      f[4] = fmaf(f[4], s1.x, h1.x); f[5] = fmaf(f[5], s1.y, h1.y); f[6] = fmaf(f[6], s1.z, h1.z); f[7] = fmaf(f[7], s1.w, h1.w);
-      if (p.act == PF_ACT_SILU) {
+      for (int u = 0; u < 4; ++u) locate(o + u * ppi, so[u], dst[u]);
 #pragma unroll
-        for (int e = 0; e < 8; ++e) f[e] = silu_f(f[e]);
-      }
-      outv = make_uint4(pack2<BF16>(f[0], f[1]), pack2<BF16>(f[2], f[3]), pack2<BF16>(f[4], f[5]), pack2<BF16>(f[6], f[7]));
+      for (int u = 0; u < 4; ++u) raw[u] = so[u] >= 0 ? __ldcg(reinterpret_cast<const uint4*>(src + so[u])) : z4;
+#pragma unroll
+      for (int u = 0; u < 4; ++u) finish(raw[u], so[u] >= 0, dst[u]);
     }
-    *dst = outv;
-  };
-  const uint4 z4 = make_uint4(0, 0, 0, 0);
-  int o = o_begin + pl;
-  for (; o + 3 * ppi < o_end; o += 4 * ppi) {  // four independent L2 loads in flight per thread
-    long long so[4];
-    uint4* dst[4];
-    uint4 raw[4];
-#pragma unroll
-    for (int u = 0; u < 4; ++u) locate(o + u * ppi, so[u], dst[u]);
-#pragma unroll
-    for (int u = 0; u < 4; ++u) raw[u] = so[u] >= 0 ? __ldcg(reinterpret_cast<const uint4*>(src + so[u])) : z4;
-#pragma unroll
-    for (int u = 0; u < 4; ++u) finish(raw[u], so[u] >= 0, dst[u]);
+    for (; o < o_end; o += ppi) {
+      long long so;
+      uint4* dst;
+      locate(o, so, dst);
+      const uint4 raw = so >= 0 ? __ldcg(reinterpret_cast<const uint4*>(src + so)) : z4;
+      finish(raw, so >= 0, dst);
+    }
   }
-  for (; o < o_end; o += ppi) {
-    long long so;
-    uint4* dst;
-    locate(o, so, dst);
-    const uint4 raw = so >= 0 ? __ldcg(reinterpret_cast<const uint4*>(src + so)) : z4;
-    finish(raw, so >= 0, dst);
-  }
-  __syncthreads();  // s_acc (scale / shift) is rewritten by the next image's phase 1
- }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -488,13 +328,11 @@ layernorm_kernel(const uint16_t* __restrict__ x, int ldx, const float* __restric
   const int vecs = C / 8;
   // affine parameters staged once per CTA in shared memory (each warp then visits many tokens)
   extern __shared__ float s_gb[];  // [2][C]
-  pdl_launch_dependents();
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {  // weights: constant during a step, safe before pdl_wait
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
     s_gb[c] = __ldg(gamma + c);
     s_gb[C + c] = __ldg(beta + c);
   }
   __syncthreads();
-  pdl_wait();
   for (int tok = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; tok < T; tok += warps_total) {
     float f[MAXV][8];
     float sum = 0.f;
@@ -557,7 +395,7 @@ layernorm_kernel(const uint16_t* __restrict__ x, int ldx, const float* __restric
 
 }  // namespace pf
 
-extern "C" int pf_groupnorm_ws_floats(int N, int groups) { return N * pf::GN_MAX_CHUNKS * groups * 2; }
+extern "C" int pf_groupnorm_ws_floats(int N, int groups) { return N * pf::GN_MAX_SLABS * groups * 2; }
 
 extern "C" int pf_groupnorm_stats(const void* x, int dtype, int N, int H, int W, int C, int ld, int groups, int circ,
                                   float eps, float* ws, int* counters, float* mean_rstd, void* stream) {
@@ -568,24 +406,23 @@ extern "C" int pf_groupnorm_stats(const void* x, int dtype, int N, int H, int W,
                    ld >= C && C / 8 <= 512,
                "pf_groupnorm_stats: bad shape N=%d H=%d W=%d C=%d ld=%d groups=%d", N, H, W, C, ld, groups);
   PF_CHECK_ARG(circ >= 0 && circ <= W, "pf_groupnorm_stats: circ=%d out of range", circ);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int hw = H * W;
-  int chunks = hw / 16;  // >= 16 pixels per CTA; small images still spread over several SMs
-  chunks = chunks < 1 ? 1 : (chunks > GN_MAX_CHUNKS ? GN_MAX_CHUNKS : chunks);
+  GnPrepParams p = {};
+  p.x1 = static_cast<const uint16_t*>(x);
+  p.ws = ws; p.mean_rstd = mean_rstd; p.counters = counters;
+  p.N = N; p.H = H; p.W = W; p.C1 = C; p.ld1 = ld; p.ld2 = ld; p.groups = groups; p.circ_stats = circ;
+  p.count = float(H) * float(W + 2 * circ) * float(C / groups);
+  p.eps = eps;
+  const int slabs = H * W / 16;  // >= 16 pixels per CTA; small images still spread over several SMs
+  p.slabs = slabs < 1 ? 1 : (slabs > GN_MAX_SLABS ? GN_MAX_SLABS : slabs);
   const int vecs = C / 8;
   int ppi = 256 / vecs;
   if (ppi < 1) ppi = 1;
-  const int threads = vecs * ppi;
-  dim3 grid(chunks, N);
   const size_t smem = 2 * (size_t)C * ppi * sizeof(float);
-  const float count = float(H) * float(W + 2 * circ) * float(C / groups);
-  if (dtype == PF_BF16)
-    launch_pdl(gn_partial_kernel<true>, grid, dim3(threads), smem, st, static_cast<const uint16_t*>(x), H, W, C, ld, groups,
-               circ, ws, counters, count, eps, mean_rstd);
-  else
-    launch_pdl(gn_partial_kernel<false>, grid, dim3(threads), smem, st, static_cast<const uint16_t*>(x), H, W, C, ld, groups,
-               circ, ws, counters, count, eps, mean_rstd);
-  PF_CHECK_LAUNCH("gn_partial_kernel");
+  const dim3 grid(p.slabs, N);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (dtype == PF_BF16) gn_prep_kernel<true, true><<<grid, vecs * ppi, smem, st>>>(p);
+  else gn_prep_kernel<false, true><<<grid, vecs * ppi, smem, st>>>(p);
+  PF_CHECK_LAUNCH("gn_prep_kernel(stats)");
   return PF_OK;
 }
 
@@ -629,22 +466,22 @@ extern "C" int pf_conv_prep(const void* x, void* out, int dtype, int N, int H, i
     set_error("pf_conv_prep: N*phases*Ho = %lld exceeds 65535", rows);
     return PF_ERR_UNSUPPORTED;
   }
-  if (dtype == PF_BF16) launch_pdl(conv_prep_kernel<true>, grid, dim3(256), smem, st, p);
-  else launch_pdl(conv_prep_kernel<false>, grid, dim3(256), smem, st, p);
+  if (dtype == PF_BF16) conv_prep_kernel<true><<<grid, 256, smem, st>>>(p);
+  else conv_prep_kernel<false><<<grid, 256, smem, st>>>(p);
   PF_CHECK_LAUNCH("conv_prep_kernel");
   return PF_OK;
 }
 
 extern "C" int pf_gn_prep_ws_floats(int N, int groups) {
-  return N * pf::GNP_MAX_SLABS * groups * 2 + N * groups * 2;
+  return N * pf::GN_MAX_SLABS * groups * 2 + N * groups * 2;
 }
 
 extern "C" int pf_gn_prep(const void* x1, int ld1, int C1, const void* x2, int ld2, int C2, void* cat_out, void* out,
                           int dtype, int N, int H, int W, int groups, float eps, const float* gamma, const float* beta,
-                          int act, int circ_stats, int circ, int up, int phases, int halo, int schedule, float* ws,
-                          int* sync, void* stream) {
+                          int act, int circ_stats, int circ, int up, int phases, int halo, float* ws, int* counters,
+                          void* stream) {
   using namespace pf;
-  PF_CHECK_ARG(x1 && out && gamma && beta && ws && sync, "pf_gn_prep: null pointer");
+  PF_CHECK_ARG(x1 && out && gamma && beta && ws && counters, "pf_gn_prep: null pointer");
   PF_CHECK_ARG(dtype == PF_BF16 || dtype == PF_F16, "pf_gn_prep: 16-bit dtype required");
   if (!x2) C2 = 0;
   const int C = C1 + C2;
@@ -666,8 +503,8 @@ extern "C" int pf_gn_prep(const void* x1, int ld1, int C1, const void* x2, int l
   p.out = static_cast<uint16_t*>(out);
   p.gamma = gamma; p.beta = beta;
   p.ws = ws;
-  p.ws_mr = ws + (size_t)N * GNP_MAX_SLABS * groups * 2;
-  p.sync = sync;
+  p.mean_rstd = ws + (size_t)N * GN_MAX_SLABS * groups * 2;
+  p.counters = counters;
   p.N = N; p.H = H; p.W = W; p.C1 = C1; p.C2 = C2; p.ld1 = ld1; p.ld2 = x2 ? ld2 : ld1; p.groups = groups; p.act = act;
   p.circ_stats = circ_stats; p.circ = circ; p.up = up; p.phases = phases; p.halo = halo;
   const int Hu = H * up, Wu = (W + 2 * circ) * up;
@@ -680,58 +517,23 @@ extern "C" int pf_gn_prep(const void* x1, int ld1, int C1, const void* x2, int l
   }
   p.count = float(H) * float(W + 2 * circ_stats) * float(C / groups);
   p.eps = eps;
-  const int hw = H * W;
-  static const int max_slabs = [] {
-    const char* e = getenv("PF_GN_SLABS");
-    const int v = e ? atoi(e) : 32;
-    return v < 1 ? 1 : (v > GNP_MAX_SLABS ? GNP_MAX_SLABS : v);
-  }();
-  static const int max_apply_ctas = [] {
-    const char* e = getenv("PF_GN_APPLY_CTAS");
-    const int v = e ? atoi(e) : 64;
-    return v < 1 ? 1 : v;
-  }();
-  int slabs = hw / 16;  // >= 16 source pixels per slab; a function of the image size ONLY (batch-invariant sums)
-  slabs = slabs < 1 ? 1 : (slabs > max_slabs ? max_slabs : slabs);
-  p.slabs = slabs;
+  const int slabs = H * W / 16;  // >= 16 source pixels per slab; a function of the image size ONLY (batch-invariant sums)
+  p.slabs = slabs < 1 ? 1 : (slabs > GN_PREP_SLABS ? GN_PREP_SLABS : slabs);
   const int vecs = C / 8;
   int ppi = 512 / vecs;
   if (ppi < 1) ppi = 1;
   const int threads = vecs * ppi;
   const size_t smem = 2 * (size_t)C * ppi * sizeof(float);  // <= 32 KB
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // Default: TWO launches — statistics with one CTA per slab, then the apply pass with up to 64 CTAs per image: the
-  // barrier's latency and the grid capped for co-residency cost more than the second launch. The fused schedule stays available (schedule = 1, or PF_GN_FUSED_MIN_N=<batch size from which to use it>).
-  static const int fused_min_n = [] {
-    const char* e = getenv("PF_GN_FUSED_MIN_N");
-    return e ? atoi(e) : (1 << 30);
-  }();
-  PF_CHECK_ARG(schedule >= 0 && schedule <= 2, "pf_gn_prep: schedule must be 0 (auto), 1 (fused) or 2 (two launches)");
-  if (schedule == 1 || (schedule == 0 && N >= fused_min_n)) {
-    // CTAs per image: the largest divisor of `slabs` that keeps the grid co-resident
-    // one CTA per SM: two such launches (2 CTAs of <= 512 threads per SM) stay co-resident
-    const int max_ctas = sm_count();
-    const int cap = max_ctas / (N < max_ctas ? N : max_ctas) > 0 ? max_ctas / (N < max_ctas ? N : max_ctas) : 1;
-    int chunks = 1;
-    for (int d = 1; d <= slabs && d <= cap; ++d)
-      if (slabs % d == 0) chunks = d;
-    const int gy = N < max_ctas / chunks ? N : max_ctas / chunks;
-    dim3 grid(chunks, gy);
-    if (dtype == PF_BF16) launch_pdl(gn_prep_kernel<true, 0>, grid, dim3(threads), smem, st, p);
-    else launch_pdl(gn_prep_kernel<false, 0>, grid, dim3(threads), smem, st, p);
-  } else {
-    dim3 g1(slabs, N);
-    if (dtype == PF_BF16) launch_pdl(gn_prep_kernel<true, 1>, g1, dim3(threads), smem, st, p);
-    else launch_pdl(gn_prep_kernel<false, 1>, g1, dim3(threads), smem, st, p);
-    PF_CHECK_LAUNCH("gn_prep_kernel(stats)");
-    const int total = phases * p.Ho * p.Wo;
-    int c2 = total / 16;  // >= 16 output positions per CTA
-    c2 = c2 < 1 ? 1 : (c2 > max_apply_ctas ? max_apply_ctas : c2);
-    dim3 g2(c2, N);
-    if (dtype == PF_BF16) launch_pdl(gn_prep_kernel<true, 2>, g2, dim3(threads), smem, st, p);
-    else launch_pdl(gn_prep_kernel<false, 2>, g2, dim3(threads), smem, st, p);
-  }
-  PF_CHECK_LAUNCH("gn_prep_kernel");
+  const dim3 g1(p.slabs, N);
+  if (dtype == PF_BF16) gn_prep_kernel<true, true><<<g1, threads, smem, st>>>(p);
+  else gn_prep_kernel<false, true><<<g1, threads, smem, st>>>(p);
+  PF_CHECK_LAUNCH("gn_prep_kernel(stats)");
+  const int ctas = p.phases * p.Ho * p.Wo / 16;  // >= 16 output positions per CTA
+  const dim3 g2(ctas < 1 ? 1 : (ctas > GN_APPLY_CTAS ? GN_APPLY_CTAS : ctas), N);
+  if (dtype == PF_BF16) gn_prep_kernel<true, false><<<g2, threads, smem, st>>>(p);
+  else gn_prep_kernel<false, false><<<g2, threads, smem, st>>>(p);
+  PF_CHECK_LAUNCH("gn_prep_kernel(apply)");
   return PF_OK;
 }
 
@@ -749,7 +551,7 @@ extern "C" int pf_layernorm(const void* x, int ldx, void* out, int ldo, int dtyp
   const uint16_t* xi = static_cast<const uint16_t*>(x);
   uint16_t* xo = static_cast<uint16_t*>(out);
   const int rounds = (C / 8 + 31) / 32;
-#define PF_LN(BF, MV) launch_pdl(layernorm_kernel<BF, MV>, dim3(blocks), dim3(256), 2 * (size_t)C * sizeof(float), st, xi, ldx, pe, pe_rows, T, C, gamma, beta, eps, xo, ldo)
+#define PF_LN(BF, MV) layernorm_kernel<BF, MV><<<blocks, 256, 2 * (size_t)C * sizeof(float), st>>>(xi, ldx, pe, pe_rows, T, C, gamma, beta, eps, xo, ldo)
   if (dtype == PF_BF16) {
     if (rounds <= 2) PF_LN(true, 2); else if (rounds <= 5) PF_LN(true, 5); else PF_LN(true, 8);
   } else {

@@ -3,7 +3,6 @@
 #include <string.h>
 
 #include "pf_common.cuh"
-#include <stdlib.h>
 
 namespace pf {
 
@@ -20,14 +19,6 @@ int check_cuda(cudaError_t e, const char* what) {
   if (e == cudaSuccess) return PF_OK;
   set_error("%s: %s (%s)", what, cudaGetErrorName(e), cudaGetErrorString(e));
   return PF_ERR_CUDA;
-}
-
-bool pdl_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("PF_PDL");  // opt-in: measured neutral inside CUDA graphs (DESIGN.md, "tried and dropped")
-    return e && e[0] == '1';
-  }();
-  return on;
 }
 
 int sm_count() {

@@ -18,8 +18,7 @@ namespace pf {
 // ----------------------------------------------------------------------------------------------
 void set_error(const char* fmt, ...);
 int  check_cuda(cudaError_t e, const char* what);
-bool pdl_enabled();  // env PF_PDL=1 (default off), pf_api.cu
-int  sm_count();     // SMs of the current device (cached; 132 on an H100 SXM when no device can be queried)
+int  sm_count();    // SMs of the current device (cached; 132 on an H100 SXM when no device can be queried)
 
 #define PF_CHECK_ARG(cond, ...)                      \
   do {                                               \
@@ -197,16 +196,6 @@ __device__ __forceinline__ float2 unpack2(uint32_t w) {
   }
 }
 
-// ---- programmatic dependent launch (PDL) -----------------------------------------------------------------
-// A denoise step is ~1000 short kernels; with plain stream order each one pays the predecessor's drain, the launch
-// latency and its own on-chip prologue (barrier init, descriptor prefetch) back to back. Kernels
-// launched through launch_pdl() may become resident as soon as every CTA of the predecessor has STARTED
-// (pdl_launch_dependents() is the first instruction), run their prologue, and block in pdl_wait() until the
-// predecessor grid has completed and its memory is visible. Rule: a kernel launched with launch_pdl() must execute
-// pdl_wait() before its first global-memory access; kernels launched with <<<>>> keep full stream-order semantics.
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
 // MUFU wrappers without the denormal range fix-ups nvcc wraps around expf / division (2 FSETP + FSEL + 3 FMUL per
 // call — the GEGLU epilogue evaluates one erf-GELU per output): results feed 16-bit stores.
 __device__ __forceinline__ float ex2_approx(float x) {
@@ -260,21 +249,5 @@ __device__ __forceinline__ float warp_max(float v) {
 }
 
 #endif  // __CUDACC__
-
-// <<<>>> replacement that allows the kernel to overlap its prologue with the predecessor's tail (see pdl_wait above)
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
-}
 
 }  // namespace pf

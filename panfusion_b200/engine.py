@@ -53,15 +53,6 @@ class _Lin:
         self.n, self.k = self.w.shape
 
 
-# LayerNorm folded into the consumer GEMM (ops.gemm_taps ln=...): A/B switch for debugging / the unfused-path tests
-FUSE_LN = __import__("os").environ.get("PF_FUSE_LN", "1") != "0"
-# GroupNorm statistics + apply + layout as ONE launch (ops.gn_prep) instead of pf_groupnorm_stats -> pf_conv_prep, and the
-# skip concatenation folded into it; same A/B switch idea
-FUSE_GN = __import__("os").environ.get("PF_FUSE_GN", "1") != "0"
-# Transformer2DModel tail: ff2 + residual + proj_out as one GEMM over [f | h] (see _Transformer.tail)
-FUSE_TAIL = __import__("os").environ.get("PF_FUSE_TAIL", "1") != "0"
-
-
 class _LinLN:
     """nn.Linear applied to LayerNorm(x): W' = gamma * W (16-bit), colsum[n] = sum_k W'[n,k] of the ROUNDED weights (so the
     mean term cancels exactly), bias' = W beta + b. `geglu_bn` packs W' for the GEGLU epilogue (value|gate per tile)."""
@@ -95,15 +86,14 @@ class _Conv3:
         self.cout, self.cin = conv.weight.shape[0], conv.weight.shape[1]
 
 
-# Upsample2D (nearest x2 + 3x3 conv) as four 2x2 phase convolutions of the original-resolution image (2.25x fewer MACs, no
-# up-sampled copy); PF_UPSAMPLE_PHASES=0 keeps the literal nearest-x2 + 9-tap path for A/B checks
-UPSAMPLE_PHASES = __import__("os").environ.get("PF_UPSAMPLE_PHASES", "1") != "0"
+class _Up:
+    """Upsample2D (nearest x2 + 3x3 conv) as four 2x2 phase convolutions of the original-resolution image (2.25x fewer
+    MACs, no up-sampled copy)."""
 
-
-class _Up(_Conv3):
     def __init__(self, conv, dev, dt):
-        super().__init__(conv, dev, dt)
         self.phase_w = [w.to(dev, dt).contiguous() for w in pack_upsample_phases(conv.weight)]
+        self.b = conv.bias.detach().to(dev, torch.float32).contiguous() if conv.bias is not None else None
+        self.cout, self.cin = conv.weight.shape[0], conv.weight.shape[1]
 
 
 class _Resnet:
@@ -120,21 +110,15 @@ class _Transformer:
         assert len(t.transformer_blocks) == 1
         self.norm = _Norm(t.norm, dev)
         self.proj_in = _Lin(t.proj_in.weight, t.proj_in.bias, dev, dt)
-        self.proj_out = _Lin(t.proj_out.weight, t.proj_out.bias, dev, dt)
         self.heads = int(blk.attn1.heads)
-        self.ln1, self.ln2, self.ln3 = _Norm(blk.norm1, dev), _Norm(blk.norm2, dev), _Norm(blk.norm3, dev)
         a1, a2 = blk.attn1, blk.attn2
-        self.qkv = _Lin(torch.cat([a1.to_q.weight, a1.to_k.weight, a1.to_v.weight], 0), None, dev, dt)
         self.out1 = _Lin(a1.to_out[0].weight, a1.to_out[0].bias, dev, dt)
-        self.q2 = _Lin(a2.to_q.weight, None, dev, dt)
         self.kv2_w = torch.cat([a2.to_k.weight, a2.to_v.weight], 0).detach()  # merged across layers by UNetPack
         self.out2 = _Lin(a2.to_out[0].weight, a2.to_out[0].bias, dev, dt)
         self.kv_off = -1
         ff1, ff2 = blk.ff.net[0].proj, blk.ff.net[2]
         self.ff1_bn = ops.pick_block_n(ff1.weight.shape[0], ops.PF_ACT_GEGLU)
-        wp, bp = pack_geglu(ff1.weight.detach(), ff1.bias.detach(), self.ff1_bn)
-        self.ff1_w, self.ff1_b = wp.to(dev, dt).contiguous(), bp.to(dev)
-        self.ff2 = _Lin(ff2.weight, ff2.bias, dev, dt)
+        self.ff_dim = ff2.weight.shape[1]  # 4C
         # ff2 and proj_out back to back are ONE linear map of [f | h]: proj_out(ff2(f) + h) = f (Wp W2)^T + h Wp^T + (Wp b2 + bp).
         # The GEGLU output f and the residual stream h are written side by side ([T, 4C | C]), so the tail of the block is a
         # single GEMM with K = 5C (same MACs, one launch and one [T, C] round trip through HBM less).
@@ -158,7 +142,6 @@ class UNetPack:
         f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()
         self.conv_in_w, self.conv_in_b = f32(unet.conv_in.weight), f32(unet.conv_in.bias)
         if not encoder_only:
-            self.conv_out_w, self.conv_out_b = f32(unet.conv_out.weight), f32(unet.conv_out.bias)
             # conv_out (C -> 4) on the tensor cores: output channels zero-padded to one 64-wide tap-GEMM tile
             co = unet.conv_out.weight.shape[0]
             wpad = torch.zeros((64, *unet.conv_out.weight.shape[1:]), dtype=unet.conv_out.weight.dtype,
@@ -166,7 +149,7 @@ class UNetPack:
             wpad[:co] = unet.conv_out.weight.detach()
             self.conv_out_packed = pack_conv3x3(wpad).to(dev, dt).contiguous()
             bpad = torch.zeros(64, dtype=torch.float32, device=dev)
-            bpad[:co] = self.conv_out_b
+            bpad[:co] = f32(unet.conv_out.bias)
             self.conv_out_bpad, self.conv_out_c = bpad, co
             self.norm_out = _Norm(unet.conv_norm_out, dev)
         te = unet.time_embedding
@@ -290,13 +273,9 @@ class Branch:
 
     def _norm_prep(self, xt: Tensor, N: int, H: int, W: int, norm: _Norm, *, act: int, circ_stats: int, circ: int,
                    halo: int) -> Tensor:
-        """GroupNorm (+SiLU) of a token tensor into the tap-GEMM A layout: one fused launch, or the two-kernel path."""
-        g = self.p.groups
-        if FUSE_GN:
-            return ops.gn_prep(xt, N, H, W, gamma=norm.g, beta=norm.b, groups=g, eps=norm.eps, act=act,
-                               circ_stats=circ_stats, circ=circ, halo=halo)
-        st = ops.groupnorm_stats(xt, N, H, W, g, norm.eps, circ_stats)
-        return ops.conv_prep(xt, N, H, W, stats=st, gamma=norm.g, beta=norm.b, groups=g, act=act, circ=circ, halo=halo)
+        """GroupNorm (+SiLU) of a token tensor into the tap-GEMM A layout."""
+        return ops.gn_prep(xt, N, H, W, gamma=norm.g, beta=norm.b, groups=self.p.groups, eps=norm.eps, act=act,
+                           circ_stats=circ_stats, circ=circ, halo=halo)
 
     def resnet(self, x: Img, r: _Resnet, skip: Optional[Img] = None) -> Img:
         """ResnetBlock2D; panorama: pad_pano(2) -> block -> unpad_pano(2) (MVGenModel.py:110-115). `skip`: the decoder's
@@ -304,15 +283,10 @@ class Branch:
         c = 2 if self.circ else 0
         N, H, W = x.N, x.H, x.W
         We = W + 2 * c
-        g = self.p.groups
         xt = x.t
-        if skip is not None:  # torch.cat([hidden, skip], 1) (MVGenModel.py:223,231): folded into the norm1 launch
-            if FUSE_GN:
-                a1, xt = ops.gn_prep(x.t, N, H, W, gamma=r.norm1.g, beta=r.norm1.b, groups=g, eps=r.norm1.eps,
-                                     act=ops.PF_ACT_SILU, circ_stats=c, circ=c, halo=1, x2=skip.t, want_cat=True)
-            else:
-                xt = self.concat(x, skip).t
-                a1 = self._norm_prep(xt, N, H, W, r.norm1, act=ops.PF_ACT_SILU, circ_stats=c, circ=c, halo=1)
+        if skip is not None:  # torch.cat([hidden, skip], 1) (MVGenModel.py:223,231): folded into the norm1 launches
+            a1, xt = ops.gn_prep(x.t, N, H, W, gamma=r.norm1.g, beta=r.norm1.b, groups=self.p.groups, eps=r.norm1.eps,
+                                 act=ops.PF_ACT_SILU, circ_stats=c, circ=c, halo=1, x2=skip.t, want_cat=True)
         else:
             a1 = self._norm_prep(xt, N, H, W, r.norm1, act=ops.PF_ACT_SILU, circ_stats=c, circ=c, halo=1)
         Hp, Wp = H + 2, We + 2
@@ -341,49 +315,24 @@ class Branch:
         d = C // t.heads
         kv = self.text_kv
         o = torch.empty((N, L, C), dtype=dt, device=dev)
-        if FUSE_LN:
-            # every LayerNorm is folded into its consumer: the producer GEMM emits per-row (sum, sum^2) partials, the
-            # consumer (gamma-scaled weights) normalises in its epilogue — the normalised tensor is never stored
-            h, st = ops.gemm_taps(xn, t.proj_in.w, new(C), M=T, Kc=t.proj_in.k, bias=t.proj_in.b, row_stats=True)
-            qkv = ops.gemm_taps(h, t.qkv_ln.w, new(3 * C), M=T, Kc=C, bias=t.qkv_ln.b,
-                                ln=(st, t.qkv_ln.colsum, t.qkv_ln.eps)).reshape(N, L, 3 * C)
-            ops.fmha(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], o, heads=t.heads, head_dim=d, scale=d ** -0.5)
-            h, st = ops.gemm_taps(o.reshape(T, C), t.out1.w, new(C), M=T, Kc=C, bias=t.out1.b, residual=h, row_stats=True)
-            q = ops.gemm_taps(h, t.q2_ln.w, new(C), M=T, Kc=C, bias=t.q2_ln.b,
-                              ln=(st, t.q2_ln.colsum, t.q2_ln.eps)).reshape(N, L, C)
-            ops.fmha(q, kv[..., t.kv_off:t.kv_off + C], kv[..., t.kv_off + C:t.kv_off + 2 * C], o, heads=t.heads,
-                     head_dim=d, scale=d ** -0.5)
-            if FUSE_TAIL and x.C == C:
-                Fk = t.ff2.k                                   # 4C
-                fh = new(Fk + C)                               # [T, f | h]: A operand of the merged ff2 + proj_out GEMM
-                h, st = ops.gemm_taps(o.reshape(T, C), t.out2.w, fh[:, Fk:], M=T, Kc=C, bias=t.out2.b, residual=h,
-                                      row_stats=True)
-                ops.gemm_taps(h, t.ff1_ln.w, fh[:, :Fk], M=T, Kc=C, bias=t.ff1_ln.b, act=ops.PF_ACT_GEGLU,
-                              block_n=t.ff1_bn, ln=(st, t.ff1_ln.colsum, t.ff1_ln.eps))
-                out = ops.gemm_taps(fh, t.tail.w, new(x.C), M=T, Kc=Fk + C, bias=t.tail.b, residual=x.t)
-                return Img(out, N, H, W)
-            h, st = ops.gemm_taps(o.reshape(T, C), t.out2.w, new(C), M=T, Kc=C, bias=t.out2.b, residual=h, row_stats=True)
-            f = ops.gemm_taps(h, t.ff1_ln.w, new(t.ff2.k), M=T, Kc=C, bias=t.ff1_ln.b, act=ops.PF_ACT_GEGLU,
-                              block_n=t.ff1_bn, ln=(st, t.ff1_ln.colsum, t.ff1_ln.eps))
-            h = ops.gemm_taps(f, t.ff2.w, new(C), M=T, Kc=t.ff2.k, bias=t.ff2.b, residual=h)
-        else:
-            h = ops.gemm_taps(xn, t.proj_in.w, new(C), M=T, Kc=t.proj_in.k, bias=t.proj_in.b)
-            # self attention
-            n1 = ops.layernorm(h, t.ln1.g, t.ln1.b, t.ln1.eps)
-            qkv = ops.gemm_taps(n1, t.qkv.w, new(3 * C), M=T, Kc=C).reshape(N, L, 3 * C)
-            ops.fmha(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], o, heads=t.heads, head_dim=d, scale=d ** -0.5)
-            h = ops.gemm_taps(o.reshape(T, C), t.out1.w, new(C), M=T, Kc=C, bias=t.out1.b, residual=h)
-            # text cross attention (K/V precomputed by set_text)
-            n2 = ops.layernorm(h, t.ln2.g, t.ln2.b, t.ln2.eps)
-            q = ops.gemm_taps(n2, t.q2.w, new(C), M=T, Kc=C).reshape(N, L, C)
-            ops.fmha(q, kv[..., t.kv_off:t.kv_off + C], kv[..., t.kv_off + C:t.kv_off + 2 * C], o, heads=t.heads,
-                     head_dim=d, scale=d ** -0.5)
-            h = ops.gemm_taps(o.reshape(T, C), t.out2.w, new(C), M=T, Kc=C, bias=t.out2.b, residual=h)
-            # feed-forward
-            n3 = ops.layernorm(h, t.ln3.g, t.ln3.b, t.ln3.eps)
-            f = ops.gemm_taps(n3, t.ff1_w, new(t.ff2.k), M=T, Kc=C, bias=t.ff1_b, act=ops.PF_ACT_GEGLU, block_n=t.ff1_bn)
-            h = ops.gemm_taps(f, t.ff2.w, new(C), M=T, Kc=t.ff2.k, bias=t.ff2.b, residual=h)
-        out = ops.gemm_taps(h, t.proj_out.w, new(x.C), M=T, Kc=C, bias=t.proj_out.b, residual=x.t)
+        # every LayerNorm is folded into its consumer: the producer GEMM emits per-row (sum, sum^2) partials, the
+        # consumer (gamma-scaled weights) normalises in its epilogue — the normalised tensor is never stored
+        h, st = ops.gemm_taps(xn, t.proj_in.w, new(C), M=T, Kc=t.proj_in.k, bias=t.proj_in.b, row_stats=True)
+        qkv = ops.gemm_taps(h, t.qkv_ln.w, new(3 * C), M=T, Kc=C, bias=t.qkv_ln.b,
+                            ln=(st, t.qkv_ln.colsum, t.qkv_ln.eps)).reshape(N, L, 3 * C)
+        ops.fmha(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], o, heads=t.heads, head_dim=d, scale=d ** -0.5)
+        h, st = ops.gemm_taps(o.reshape(T, C), t.out1.w, new(C), M=T, Kc=C, bias=t.out1.b, residual=h, row_stats=True)
+        q = ops.gemm_taps(h, t.q2_ln.w, new(C), M=T, Kc=C, bias=t.q2_ln.b,
+                          ln=(st, t.q2_ln.colsum, t.q2_ln.eps)).reshape(N, L, C)
+        ops.fmha(q, kv[..., t.kv_off:t.kv_off + C], kv[..., t.kv_off + C:t.kv_off + 2 * C], o, heads=t.heads,
+                 head_dim=d, scale=d ** -0.5)
+        Fk = t.ff_dim
+        fh = new(Fk + C)  # [T, f | h]: A operand of the merged ff2 + proj_out GEMM
+        h, st = ops.gemm_taps(o.reshape(T, C), t.out2.w, fh[:, Fk:], M=T, Kc=C, bias=t.out2.b, residual=h,
+                              row_stats=True)
+        ops.gemm_taps(h, t.ff1_ln.w, fh[:, :Fk], M=T, Kc=C, bias=t.ff1_ln.b, act=ops.PF_ACT_GEGLU, block_n=t.ff1_bn,
+                      ln=(st, t.ff1_ln.colsum, t.ff1_ln.eps))
+        out = ops.gemm_taps(fh, t.tail.w, new(x.C), M=T, Kc=Fk + C, bias=t.tail.b, residual=x.t)
         return Img(out, N, H, W)
 
     def downsample(self, x: Img, d: _Conv3) -> Img:
@@ -408,14 +357,6 @@ class Branch:
         4-tap GEMMs over the zero-haloed original image, each scattering its phase into the 2x larger output."""
         c = 1 if self.circ else 0
         N, H, W = x.N, x.H, x.W
-        if not UPSAMPLE_PHASES:
-            a = ops.conv_prep(x.t, N, H, W, circ=c, up=2, halo=1)
-            Hu, Wu = 2 * H, 2 * (W + 2 * c)
-            Hp, Wp = Hu + 2, Wu + 2
-            out = torch.empty((N * Hu * 2 * W, u.cout), dtype=self.dt, device=x.t.device)
-            ops.gemm_taps(a, u.w, out, M=N * Hp * Wp, Kc=u.cin, taps=taps3x3(Wp), bias=u.b,
-                          image_map=(Hp, Wp, 1, 1 + 2 * c, Hu, 2 * W))
-            return Img(out, N, Hu, 2 * W)
         a = ops.conv_prep(x.t, N, H, W, circ=c, up=1, halo=1)
         Hp, Wp = H + 2, W + 2 * c + 2
         out = torch.empty((N * 2 * H * 2 * W, u.cout), dtype=self.dt, device=x.t.device)
@@ -427,14 +368,6 @@ class Branch:
                               image_map=(Hp, Wp, 1, 1 + c, H, W), scatter=(2, 2, pa, pb))
                 k += 1
         return Img(out, N, 2 * H, 2 * W)
-
-    def concat(self, a: Img, b: Img) -> Img:
-        """torch.cat([hidden, skip], dim=1) in channels-last layout."""
-        T = a.t.shape[0]
-        out = torch.empty((T, a.C + b.C), dtype=self.dt, device=a.t.device)
-        ops.copy2d(a.t, out[:, :a.C])
-        ops.copy2d(b.t, out[:, a.C:])
-        return Img(out, a.N, a.H, a.W)
 
 
 # ---- ControlNet (BASELINE config 5) ------------------------------------------------------------------------------

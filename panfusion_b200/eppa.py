@@ -15,9 +15,7 @@ import torch.nn as nn
 from torch import Tensor
 
 from . import geometry, ops
-from . import engine
 from .engine import Img, _Lin, _LinLN, _Norm, img_from_nchw
-from .packing import pack_geglu
 
 
 class _CrossAttention(nn.Module):  # parameters of models/modules/transformer.py:41-56
@@ -68,36 +66,25 @@ def pack_block(t: _Block, dev, dt) -> dict:
     """The weights of a _Block packed for the kernels (once per device/dtype)."""
     a = t.attn1
     bn = ops.pick_block_n(t.ff.net[0].proj.weight.shape[0], ops.PF_ACT_GEGLU)
-    wp, bp = pack_geglu(t.ff.net[0].proj.weight.detach(), t.ff.net[0].proj.bias.detach(), bn)
     return dict(
         key=(dev, dt),
         qkv=_Lin(torch.cat([a.to_q.weight, a.to_k.weight, a.to_v.weight], 0), None, dev, dt),
         out=_Lin(a.to_out.weight, a.to_out.bias, dev, dt),
-        ff1_w=wp.to(dev, dt).contiguous(), ff1_b=bp.to(dev), ff1_bn=bn,
+        ff1_bn=bn,
         ff2=_Lin(t.ff.net[2].weight, t.ff.net[2].bias, dev, dt),
         ff1_ln=_LinLN(t.ff.net[0].proj.weight, t.ff.net[0].proj.bias, t.norm2, dev, dt, geglu_bn=bn),
-        ln1=_Norm(t.norm1, dev), ln2=_Norm(t.norm2, dev), heads=a.heads)
+        ln1=_Norm(t.norm1, dev), heads=a.heads)
 
 
 def block_tail(w: dict, o: Tensor, x_tok: Tensor, rows: int) -> Tensor:
-    """to_out(o) + x, then x + FF(norm2(x)) (transformer.py:159-160) on [rows, C] tokens; w = pack_block(...)."""
+    """to_out(o) + x, then x + FF(norm2(x)) (transformer.py:159-160) on [rows, C] tokens; w = pack_block(...).
+    norm2 is folded into the GEGLU projection (engine._LinLN)."""
     C = w["out"].n
     new = lambda r, n: torch.empty((r, n), dtype=x_tok.dtype, device=x_tok.device)
-    if engine.FUSE_LN:  # norm2 folded into the GEGLU projection (engine._LinLN)
-        x1, st = ops.gemm_taps(o, w["out"].w, new(rows, C), M=rows, Kc=C, bias=w["out"].b, residual=x_tok,
-                               row_stats=True)
-        f = ops.gemm_taps(x1, w["ff1_ln"].w, new(rows, 4 * C), M=rows, Kc=C, bias=w["ff1_ln"].b,
-                          act=ops.PF_ACT_GEGLU, block_n=w["ff1_bn"], ln=(st, w["ff1_ln"].colsum, w["ff1_ln"].eps))
-        return ops.gemm_taps(f, w["ff2"].w, new(rows, C), M=rows, Kc=4 * C, bias=w["ff2"].b, residual=x1)
-    x1 = ops.gemm_taps(o, w["out"].w, new(rows, C), M=rows, Kc=C, bias=w["out"].b, residual=x_tok)
-    n2 = ops.layernorm(x1, w["ln2"].g, w["ln2"].b, w["ln2"].eps)
-    f = ops.gemm_taps(n2, w["ff1_w"], new(rows, 4 * C), M=rows, Kc=C, bias=w["ff1_b"], act=ops.PF_ACT_GEGLU,
-                      block_n=w["ff1_bn"])
+    x1, st = ops.gemm_taps(o, w["out"].w, new(rows, C), M=rows, Kc=C, bias=w["out"].b, residual=x_tok, row_stats=True)
+    f = ops.gemm_taps(x1, w["ff1_ln"].w, new(rows, 4 * C), M=rows, Kc=C, bias=w["ff1_ln"].b, act=ops.PF_ACT_GEGLU,
+                      block_n=w["ff1_bn"], ln=(st, w["ff1_ln"].colsum, w["ff1_ln"].eps))
     return ops.gemm_taps(f, w["ff2"].w, new(rows, C), M=rows, Kc=4 * C, bias=w["ff2"].b, residual=x1)
-
-
-# resident form of the correspondence bias: tile-packed (only non-constant 128 x 64 tiles) unless PF_EPPA_DENSE_BIAS=1
-PACK_BIAS = __import__("os").environ.get("PF_EPPA_DENSE_BIAS", "0") == "0"
 
 
 class CameraTables:
@@ -221,8 +208,8 @@ class CameraTables:
             # per-view query count is not a multiple of the 128-row tile (the 8x8 level) cannot be sliced by view shard and
             # stays dense (it is tiny).
             P, E = ph * pw, eh * ew
-            d1 = ("packed", *ops.bias_pack_tiles(b1)) if (PACK_BIAS and E % 128 == 0) else ("dense", b1, ops.bias_tile_flags(b1))
-            d2 = ("packed", *ops.bias_pack_tiles(b2)) if (PACK_BIAS and P % 128 == 0) else ("dense", b2, ops.bias_tile_flags(b2))
+            d1 = ("packed", *ops.bias_pack_tiles(b1)) if E % 128 == 0 else ("dense", b1, ops.bias_tile_flags(b1))
+            d2 = ("packed", *ops.bias_pack_tiles(b2)) if P % 128 == 0 else ("dense", b2, ops.bias_tile_flags(b2))
             self._bias[k] = (d1, d2)
         return self._bias[k]
 

@@ -20,9 +20,6 @@ from .engine import Branch, ControlBranch, ControlNetPack, Img, UNetPack
 from .eppa import CameraTables, WarpAttn
 
 
-_EPPA_SPLIT = __import__("os").environ.get("PF_EPPA_SPLIT", "1") != "0"  # A/B switch (scripts only)
-
-
 class MultiViewBaseModel(nn.Module):
     def __init__(self, unet, pano_unet, pers_cn=None, pano_cn=None, pano_pad=True, compute_dtype=torch.bfloat16,
                  overlap_branches=True):
@@ -146,8 +143,8 @@ class MultiViewBaseModel(nn.Module):
         two = bool(self.overlap_branches and has_pers)
         if two and self._side is None:
             # the panorama branch (many small launches that every fusion waits for) runs at higher stream priority: 25.9 -> 25.7 ms
-            # single GPU, 9.60 -> 9.55 ms for a rank of the 8-GPU layout (PF_SIDE_PRIORITY=0 restores equal priorities)
-            self._side = torch.cuda.Stream(device=dev, priority=int(__import__("os").environ.get("PF_SIDE_PRIORITY", "-1")))
+            # single GPU, 9.60 -> 9.55 ms for a rank of the 8-GPU layout
+            self._side = torch.cuda.Stream(device=dev, priority=-1)
         side = self._side if two else main
         keep = []  # tensors produced on `main` but consumed on `side`: kept alive until the next join
 
@@ -164,12 +161,7 @@ class MultiViewBaseModel(nn.Module):
             join()
             # direction 1 of the fusion continues on the side stream and feeds the panorama branch there; direction 2
             # stays on the main stream: after the block the two streams are already forked again
-            split = two and _EPPA_SPLIT
-            h, p = block.forward_tokens(h, p, cam_key, par, side=side if split else None, keep=keep)
-            if not split:
-                keep.append(p.t)
-                fork()
-            return h, p
+            return block.forward_tokens(h, p, cam_key, par, side=side if two else None, keep=keep)
 
         fork()
         # ControlNets (MVGenModel.py:66-83): black-box encoder passes on the UN-padded latents; their outputs are only

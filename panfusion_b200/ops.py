@@ -261,14 +261,11 @@ def conv_prep(x: Tensor, N: int, H: int, W: int, *, stats: Optional[Tensor] = No
     return out
 
 
-GN_FUSED_MIN_N = int(__import__("os").environ.get("PF_GN_FUSED_MIN_N", str(1 << 30)))  # mirrors the switch inside pf_gn_prep
-
-
 def gn_prep(x: Tensor, N: int, H: int, W: int, *, gamma: Tensor, beta: Tensor, groups: int, eps: float,
             act: int = PF_ACT_NONE, circ_stats: int = 0, circ: int = 0, up: int = 1, phases: int = 1, halo: int = 1,
-            x2: Optional[Tensor] = None, want_cat: bool = False, schedule: int = 0):
-    """GroupNorm statistics + apply (+SiLU) + conv_prep layout in one launch (pf_gn_prep); with x2 the normalised tensor
-    is the channel concatenation cat(x, x2) and want_cat also returns that raw concatenation.
+            x2: Optional[Tensor] = None, want_cat: bool = False):
+    """GroupNorm statistics + apply (+SiLU) + conv_prep layout (pf_gn_prep: a statistics and an apply launch); with x2
+    the normalised tensor is the channel concatenation cat(x, x2) and want_cat also returns that raw concatenation.
     -> out [phases * N * Ho * Wo, C] (and cat [N*H*W, C] if want_cat)."""
     C1, C2 = x.shape[1], (x2.shape[1] if x2 is not None else 0)
     Cc = C1 + C2
@@ -281,11 +278,10 @@ def gn_prep(x: Tensor, N: int, H: int, W: int, *, gamma: Tensor, beta: Tensor, g
     out = torch.empty((phases * N * Ho * Wo, Cc), dtype=x.dtype, device=x.device)
     cat = torch.empty((N * H * W, Cc), dtype=x.dtype, device=x.device) if want_cat else None
     ws = torch.empty(lib.pf_gn_prep_ws_floats(N, groups), dtype=torch.float32, device=x.device)
-    _count(1 if (schedule == 1 or (schedule == 0 and N >= GN_FUSED_MIN_N)) else 2)
+    _count(2)
     _lib.check(lib.pf_gn_prep(_vp(x), x.stride(0), C1, _vp(x2), x2.stride(0) if x2 is not None else 0, C2, _vp(cat),
                               _vp(out), _lib.dtype_code(x.dtype), N, H, W, groups, _f(eps), _vp(gamma), _vp(beta), act,
-                              circ_stats, circ, up, phases, halo, schedule, _vp(ws),
-                              _vp(_gn_counter_slot(x.device, 3 * N)), _st()))
+                              circ_stats, circ, up, phases, halo, _vp(ws), _vp(_gn_counter_slot(x.device, N)), _st()))
     return (out, cat) if want_cat else out
 
 
@@ -309,17 +305,6 @@ def conv_in(x: Tensor, w: Tensor, b: Optional[Tensor], dtype: torch.dtype, circ:
     _count(1)
     _lib.check(_lib.lib().pf_conv_in(_vp(x), _vp(w), _vp(b), _vp(out), _lib.dtype_code(dtype), N, Cin, H, W, Cout,
                                      int(circ), int(act), _st()))
-    return out
-
-
-def conv_out(xp: Tensor, N: int, H: int, W: int, w: Tensor, b: Optional[Tensor], circ: int) -> Tensor:
-    """xp = conv_prep(.., GroupNorm + SiLU, circ, halo=1) [N*(H+2)*(W+2*circ+2), C] -> NCHW fp32 [N, Cout, H, W]."""
-    Cc, Cout = xp.shape[1], w.shape[0]
-    assert xp.shape[0] == N * (H + 2) * (W + 2 * circ + 2) and xp.is_contiguous()
-    out = torch.empty((N, Cout, H, W), dtype=torch.float32, device=xp.device)
-    _count(1)
-    _lib.check(_lib.lib().pf_conv_out(_vp(xp), _lib.dtype_code(xp.dtype), _vp(w), _vp(b), _vp(out), N, H, W, Cc, Cout,
-                                      int(circ), _st()))
     return out
 
 

@@ -6,10 +6,11 @@ Reference: `decode_latent` models/pano/PanoGenerator.py:272-278, the padded pano
 (`pad_pano(latent=True)` with `latent_pad = 8`, PanoGenerator.py:227-238), `tensor_to_image`
 models/modules/utils.py:9-15. The decoder is diffusers `AutoencoderKL` [3P]; like the UNets it is consumed by
 attribute walk to read its parameters once (`VAEDecoder.prepare`) and then runs on the kernels of the denoiser:
-conv_in on `pf_conv_in`, every 3x3 conv / shortcut / linear on the tap-GEMM, GroupNorm + SiLU + zero halo + nearest x2
-in `pf_groupnorm_stats` / `pf_conv_prep`. The mid-block attention has one head of width 512 — outside the flash
-kernel's head sizes and 0.1 % of the decoder's FLOPs — and runs as tap-GEMM (Q K^T, fp32) -> `pf_softmax_rows` ->
-tap-GEMM (P V^T-operand). No PyTorch compute fallback.
+conv_in on `pf_conv_in`, every 3x3 conv / shortcut / linear on the tap-GEMM (Upsample2D as four phase convolutions),
+GroupNorm + SiLU + zero halo in `pf_groupnorm_stats` (the statistics launch of `pf_gn_prep`) / `pf_conv_prep`. The
+mid-block attention has one head of width 512 — outside the flash kernel's head sizes and 0.1 % of the decoder's
+FLOPs — and runs as tap-GEMM (Q K^T, fp32) -> `pf_softmax_rows` -> tap-GEMM (P V^T-operand). No PyTorch compute
+fallback.
 """
 from __future__ import annotations
 

@@ -230,8 +230,8 @@ def test_layernorm_fused_into_geglu(cuda_device, dtype, M, C, sched):
 @pytest.mark.parametrize("circ", [False, True])
 def test_upsample_phase_convolutions(cuda_device, dtype, circ):
     """Upsample2D (nearest x2 -> conv3x3, MVGenModel.py:272-277; panorama: pad_pano(1) -> up -> unpad_pano(2)) as four
-    2x2 phase convolutions with scattered output (pf_gemm_args.out_sy/out_sx) == the torch composition, and == the literal
-    nearest-x2 + 9-tap path up to the rounding of the pre-summed weights."""
+    2x2 phase convolutions with scattered output (pf_gemm_args.out_sy/out_sx) == the torch composition, up to the
+    rounding of the pre-summed weights."""
     from oracle.eppa import pad_pano
     from panfusion_b200 import engine
     N, C, Co, H, W = 3, 128, 192, 8, 12
@@ -250,16 +250,7 @@ def test_upsample_phase_convolutions(cuda_device, dtype, circ):
     br = engine.Branch.__new__(engine.Branch)
     br.p, br.circ, br.dt = _P(), circ, dtype
     u = engine._Up(conv, cuda_device, dtype)
-    xt = engine.img_from_nchw(x.to(cuda_device), dtype)
-    outs = {}
-    for phases in (True, False):
-        engine.UPSAMPLE_PHASES = phases
-        try:
-            o = br.upsample(xt, u)
-        finally:
-            engine.UPSAMPLE_PHASES = True
-        assert (o.N, o.H, o.W) == (N, 2 * H, 2 * W)
-        outs[phases] = o.nchw().float().cpu()
+    o = br.upsample(engine.img_from_nchw(x.to(cuda_device), dtype), u)
+    assert (o.N, o.H, o.W) == (N, 2 * H, 2 * W)
     tol = dict(rtol=2 ** -7, atol=3e-2) if dtype == torch.bfloat16 else dict(rtol=2 ** -10, atol=4e-3)
-    torch.testing.assert_close(outs[True], ref, **tol)
-    torch.testing.assert_close(outs[False], ref, **tol)
+    torch.testing.assert_close(o.nchw().float().cpu(), ref, **tol)

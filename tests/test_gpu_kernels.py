@@ -2,6 +2,7 @@
 timestep embedding) against plain PyTorch fp32 on the same 16-bit-rounded inputs, and the EPPA tables against the
 oracle's get_masks / get_coords / SphericalPE (models/pano/utils.py:10-106, transformer.py:185-201)."""
 import math
+from types import SimpleNamespace
 
 import numpy as np
 import pytest
@@ -69,11 +70,11 @@ def test_conv_prep(cuda_device, circ, up, phases, halo):
     (1, 640, 320, 16, 32, 2, 2, 1, "silu"),    # the same on the panorama branch
     (20, 64, 64, 4, 4, 0, 0, 1, "silu"),       # many tiny images: one CTA per image
 ])
-def test_gn_prep_fused(cuda_device, dtype, N, C1, C2, H, W, circ_stats, circ, halo, act):
-    """pf_gn_prep (statistics + apply + layout + skip concatenation in one launch, per-image barrier inside) against the
-    torch composition pad_pano -> GroupNorm -> SiLU -> pad of the reference (MVGenModel.py:110-115,223-231; diffusers
-    ResnetBlock2D norm1/norm2) and against the two-kernel path; the raw concatenation output is exact. Launched 3
-    times in a row: the barrier words must re-arm themselves."""
+def test_gn_prep(cuda_device, dtype, N, C1, C2, H, W, circ_stats, circ, halo, act):
+    """pf_gn_prep (statistics + apply + layout + skip concatenation) against the torch composition pad_pano -> GroupNorm
+    -> SiLU -> pad of the reference (MVGenModel.py:110-115,223-231; diffusers ResnetBlock2D norm1/norm2) and against
+    pf_groupnorm_stats -> pf_conv_prep; the raw concatenation output is exact. Launched 3 times in a row with the same
+    bits each time: the per-image counters must re-arm themselves."""
     from panfusion_b200 import ops
     from oracle.eppa import pad_pano
     g = torch.Generator().manual_seed(N + C1 + C2 + H)
@@ -98,8 +99,8 @@ def test_gn_prep_fused(cuda_device, dtype, N, C1, C2, H, W, circ_stats, circ, ha
     kw = dict(gamma=gamma.to(dev), beta=beta.to(dev), groups=32, eps=1e-5,
               act=ops.PF_ACT_SILU if act == "silu" else ops.PF_ACT_NONE, circ_stats=circ_stats, circ=circ, halo=halo)
     outs = []
-    for sched in (1, 2, 1, 2, 0):  # fused launch / statistics + apply launches, alternating: same bits, barrier words re-armed
-        r = ops.gn_prep(x1, N, H, W, x2=x2, want_cat=bool(C2), schedule=sched, **kw)
+    for _ in range(3):
+        r = ops.gn_prep(x1, N, H, W, x2=x2, want_cat=bool(C2), **kw)
         got, cat = r if C2 else (r, None)
         outs.append(got.clone())
     torch.cuda.synchronize()
@@ -130,8 +131,9 @@ def test_layernorm(cuda_device, T, C, with_pe):
 
 
 @pytest.mark.parametrize("circ", [False, True])
-def test_conv_in_out(cuda_device, circ):
-    from panfusion_b200 import ops
+def test_conv_in_and_branch_conv_out(cuda_device, circ):
+    from panfusion_b200 import engine, ops
+    from panfusion_b200.packing import pack_conv3x3
     from oracle.eppa import pad_pano, unpad_pano
     g = torch.Generator().manual_seed(4)
     N, H, W, C = 2, 16, 32, 320
@@ -141,17 +143,22 @@ def test_conv_in_out(cuda_device, circ):
     ref = conv(lat, w_in, b_in)
     got = ops.conv_in(lat.to(cuda_device), w_in.to(cuda_device), b_in.to(cuda_device), torch.float16, circ)
     torch.testing.assert_close(got.float().cpu().reshape(N, H, W, C).permute(0, 3, 1, 2), ref, rtol=1e-3, atol=2e-3)
-    # conv_norm_out -> SiLU -> conv_out
+    # conv_norm_out -> SiLU -> conv_out, as Branch.conv_out runs it: pf_gn_prep, then the 64-wide tap-GEMM
     x = torch.randn(N, C, H, W, generator=g).half()
     gamma, beta = torch.randn(C, generator=g), torch.randn(C, generator=g)
     w_out, b_out = torch.randn(4, C, 3, 3, generator=g) * 0.05, torch.randn(4, generator=g)
     ref = conv(F.silu(F.group_norm(x.float(), 32, gamma, beta, 1e-5)), w_out, b_out)
-    xt = _tokens(x).to(cuda_device)
-    stats = ops.groupnorm_stats(xt, N, H, W, 32, 1e-5, 0)
-    xp = ops.conv_prep(xt, N, H, W, stats=stats, gamma=gamma.to(cuda_device), beta=beta.to(cuda_device), groups=32,
-                       act=ops.PF_ACT_SILU, circ=int(circ), halo=1)
-    got = ops.conv_out(xp, N, H, W, w_out.to(cuda_device), b_out.to(cuda_device), int(circ))
-    torch.testing.assert_close(got.cpu(), ref, rtol=2e-3, atol=3e-3)  # the prepared activations are rounded to fp16
+    # the fields of engine.UNetPack that Branch.conv_out reads: 4 output channels zero-padded to one 64-wide tile
+    wpad, bpad = torch.zeros(64, C, 3, 3), torch.zeros(64)
+    wpad[:4], bpad[:4] = w_out, b_out
+    norm = SimpleNamespace(weight=gamma, bias=beta, eps=1e-5, num_groups=32)
+    pack = SimpleNamespace(dt=torch.float16, groups=32, norm_out=engine._Norm(norm, cuda_device), conv_out_c=4,
+                           conv_out_packed=pack_conv3x3(wpad).to(cuda_device, torch.float16).contiguous(),
+                           conv_out_bpad=bpad.to(cuda_device))
+    br = engine.Branch(pack, circular=circ)
+    got = br.conv_out(engine.img_from_nchw(x.to(cuda_device), torch.float16))
+    # the prepared activations and the packed weights are rounded to fp16
+    torch.testing.assert_close(got.cpu(), ref, rtol=2e-3, atol=3e-3)
 
 
 @pytest.mark.parametrize("W", [32, 30])  # 4-pixel register-blocked path and the generic one

@@ -37,3 +37,21 @@ def test_gpu_tests_are_marked():
     for p in (ROOT / "tests").glob("test_*.py"):
         if not p.name.startswith("test_gpu_") and p.name != Path(__file__).name:
             assert "cuda_device" not in p.read_text(), f"{p.name} uses a GPU fixture but is not a test_gpu_ file"
+
+
+def test_environment_variables_read_by_the_library():
+    """Every layer has one code path: the library reads no environment switch besides these (split-K on/off for the
+    bit-identical sharded check, the multi-GPU transport and its forced fallback, the library path, the compiler)."""
+    allowed = {"PF_SPLIT_K", "PF_DEVICE_GATHER", "PF_FORCE_IPC_FAIL", "PF_LIB_PATH", "NVCC"}
+    read, opaque = set(), []
+    for p in PKG.rglob("*"):
+        if p.suffix not in (".py", ".cu", ".cuh", ".h") or "__pycache__" in p.parts:
+            continue
+        for m in re.finditer(r"\b(environ|getenv)\b(.{0,40})", p.read_text()):
+            name = re.match(r"""\s*(?:\.get\s*\(|\[|\()\s*["'](\w+)["']""", m.group(2))
+            if name:
+                read.add(name.group(1))
+            else:
+                opaque.append(f"{p.relative_to(ROOT)}: {m.group(0)}")
+    assert not opaque, f"environment read without a literal name: {opaque}"
+    assert read == allowed, f"unexpected: {sorted(read - allowed)}, not found: {sorted(allowed - read)}"
