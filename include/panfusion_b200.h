@@ -68,6 +68,24 @@ int pf_e2p_shared(const void* src, void* dst, int dtype, int B, int src_repeat, 
 int pf_e2p_py360(const void* src, void* dst, int is_u8, int H, int W, int C, int h, int w, const double* cams,
                  int num_cams, int mode, void* stream);
 
+/* py360convert.c2e (external/py360convert/c2e.py:6-64, utils.py:40-64,135-173): horizon cube cube[face_w, 6*face_w, C]
+ * (faces F R B L U D, uint8 when is_u8, else fp32) -> dst[h, w, C] float64, the dtype the reference returns (its padded
+ * faces are float64). w must be a multiple of 8 (c2e.py:26). Face coordinates in float32 as numpy computes them, clip /
+ * scale / bilinear weights in float64, scipy 'wrap' sampling of the (face_w + 2)-padded faces.
+ *   ceil_rows[w / 4]: the ceiling row of each column of one quarter (equirect_facetype: h // 2 - round(arctan(cos(lon))
+ *                     * h / pi) in float64 on the host), device memory.
+ *   border[6][4 * face_w + 4]: horizon-cube pixel index (row * 6 * face_w + col) of every pad sample of each face, -1 for
+ *                     a zero pad: [row face_w][face_w], [row face_w + 1][face_w], [col face_w][face_w + 2],
+ *                     [col face_w + 1][face_w + 2]; device memory. panfusion_b200/py360.py builds both tables.
+ * mode: 0 bilinear, 1 nearest; anything else is PF_ERR_UNSUPPORTED. */
+int pf_c2e_py360(const void* cube, double* dst, int is_u8, int face_w, int C, int h, int w, const int* ceil_rows,
+                 const int* border, int mode, void* stream);
+
+/* py360convert.e2c (external/py360convert/e2c.py:6-40): src[H, W, C] (uint8 when is_u8, else fp32) -> horizon cube
+ * dst[face_w, 6 * face_w, C] in the source dtype; the grid (xyzcube -> xyz2uv -> uv2coor) in float32, sampled like
+ * pf_e2p_py360 (integers rounded half up). mode: 0 bilinear, 1 nearest; anything else is PF_ERR_UNSUPPORTED. */
+int pf_e2c_py360(const void* src, void* dst, int is_u8, int H, int W, int C, int face_w, int mode, void* stream);
+
 /* p2e(p_img[B,C,hp,wp]) -> equi[B,C,He,We] (already multiplied by mask), mask[B,1,He,We] uint8 (may be NULL)
  * (p2e.py:52-77; grid math p2e.py:9-49) */
 int pf_p2e(const void* src, void* dst, uint8_t* mask, int dtype, int B, int C, int hp, int wp, int He, int We,

@@ -81,7 +81,7 @@ def lib() -> C.CDLL:
 # every symbol include/panfusion_b200.h declares (checked by tests/test_cabi.py against the header text)
 EXPORTS = [
     "pf_last_error", "pf_version", "pf_check_device",
-    "pf_e2p", "pf_e2p_shared", "pf_e2p_py360", "pf_p2e",
+    "pf_e2p", "pf_e2p_shared", "pf_e2p_py360", "pf_c2e_py360", "pf_e2c_py360", "pf_p2e",
     "pf_gemm_taps", "pf_gemm_pick_block_n", "pf_gemm_splitk_plan", "pf_gemm_row_stats_slots",
     "pf_fmha_fwd", "pf_bias_tile_flags", "pf_bias_tile_scan", "pf_bias_tile_pack",
     "pf_groupnorm_ws_floats", "pf_groupnorm_stats", "pf_conv_prep", "pf_gn_prep_ws_floats", "pf_gn_prep", "pf_layernorm",

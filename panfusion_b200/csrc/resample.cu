@@ -424,33 +424,13 @@ __device__ __forceinline__ long long py360_src_index(int r, int x, int H, int W)
   return (long long)(r == H ? H - 1 : 0) * W + xr;
 }
 
+// utils.py:125-132 sample_equirec: scipy map_coordinates([cy, cx], order 1 or 0, mode='wrap') over the equirect image
+// with its two pole rows appended, every channel of one output pixel. Shared by e2p and e2c.
 template <typename T>
-__global__ void __launch_bounds__(256)
-e2p_py360_kernel(const T* __restrict__ src, T* __restrict__ dst, int H, int W, int C, int h, int w,
-                 const double* __restrict__ cams, int nearest) {
-  const int cam_i = blockIdx.y;
-  const int pix = blockIdx.x * blockDim.x + threadIdx.x;
-  if (pix >= h * w) return;
-  const int i = pix / w, j = pix - i * w;
-  const double* cam = cams + (size_t)cam_i * PF_CAM360_DOUBLES;
-  // xyzpers: float32 linspace grids, z = 1, then three float64 rotations applied to the ROW vector
-  double v[3] = {double(float(np_linspace(-cam[27], cam[27], w, j))), -double(float(np_linspace(-cam[28], cam[28], h, i))), 1.0};
-#pragma unroll
-  for (int r = 0; r < 3; ++r) {
-    const double* R = cam + 9 * r;
-    double o[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k)
-      o[k] = __dadd_rn(__dadd_rn(__dmul_rn(v[0], R[k]), __dmul_rn(v[1], R[3 + k])), __dmul_rn(v[2], R[6 + k]));
-    v[0] = o[0]; v[1] = o[1]; v[2] = o[2];
-  }
-  const double uu = atan2(v[0], v[2]);
-  const double vv = atan2(v[1], sqrt(v[0] * v[0] + v[2] * v[2]));
-  const double cx = (uu / (2.0 * M_PI) + 0.5) * double(W) - 0.5;
-  const double cy = (-vv / M_PI + 0.5) * double(H) - 0.5;
+__device__ __forceinline__ void py360_sample_equirec(const T* __restrict__ src, int H, int W, int C, double cx,
+                                                     double cy, int nearest, T* __restrict__ out) {
   const int HP = H + 2;
   const double y = py360_wrap(cy, HP), x = py360_wrap(cx, W);
-  T* out = dst + ((size_t)cam_i * h * w + pix) * C;
   if (nearest) {
     int yi = int(floor(y + 0.5)), xi = int(floor(x + 0.5));
     if (yi > HP - 1) yi -= HP - 1;
@@ -481,6 +461,147 @@ e2p_py360_kernel(const T* __restrict__ src, T* __restrict__ dst, int H, int W, i
   }
 }
 
+template <typename T>
+__global__ void __launch_bounds__(256)
+e2p_py360_kernel(const T* __restrict__ src, T* __restrict__ dst, int H, int W, int C, int h, int w,
+                 const double* __restrict__ cams, int nearest) {
+  const int cam_i = blockIdx.y;
+  const int pix = blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= h * w) return;
+  const int i = pix / w, j = pix - i * w;
+  const double* cam = cams + (size_t)cam_i * PF_CAM360_DOUBLES;
+  // xyzpers: float32 linspace grids, z = 1, then three float64 rotations applied to the ROW vector
+  double v[3] = {double(float(np_linspace(-cam[27], cam[27], w, j))), -double(float(np_linspace(-cam[28], cam[28], h, i))), 1.0};
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    const double* R = cam + 9 * r;
+    double o[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+      o[k] = __dadd_rn(__dadd_rn(__dmul_rn(v[0], R[k]), __dmul_rn(v[1], R[3 + k])), __dmul_rn(v[2], R[6 + k]));
+    v[0] = o[0]; v[1] = o[1]; v[2] = o[2];
+  }
+  const double uu = atan2(v[0], v[2]);
+  const double vv = atan2(v[1], sqrt(v[0] * v[0] + v[2] * v[2]));
+  const double cx = (uu / (2.0 * M_PI) + 0.5) * double(W) - 0.5;
+  const double cy = (-vv / M_PI + 0.5) * double(H) - 0.5;
+  py360_sample_equirec(src, H, W, C, cx, cy, nearest, dst + ((size_t)cam_i * h * w + pix) * C);
+}
+
+// numpy float32 math restated on the device: each float32 ufunc result is the float64 function rounded to float
+// (correctly rounded but for rare double-rounding ties; numpy's own float32 kernels are within about one ulp of that).
+__device__ __forceinline__ float f32_tan(float a) { return float(tan(double(a))); }
+__device__ __forceinline__ float f32_sin(float a) { return float(sin(double(a))); }
+__device__ __forceinline__ float f32_cos(float a) { return float(cos(double(a))); }
+__device__ __forceinline__ float f32_atan2(float y, float x) { return float(atan2(double(y), double(x))); }
+
+// np.linspace(start, stop, n, dtype=float32)[i]: float64 i * step, then + start, each rounded (no contraction into
+// an FMA), then cast to float32; the last sample is `stop` exactly.
+__device__ __forceinline__ float np_linspace_f32(double start, double stop, int n, int i) {
+  if (n == 1) return float(start);
+  if (i == n - 1) return float(stop);
+  return float(__dadd_rn(__dmul_rn(double(i), (stop - start) / double(n - 1)), start));
+}
+
+// e2c.py:6-40: thread <-> one pixel of the horizon cube [fw, 6 fw, C]. xyzcube -> xyz2uv -> uv2coor in float32
+// (utils.py:5-37,82-114), then the e2p sampler.
+template <typename T>
+__global__ void __launch_bounds__(256)
+e2c_py360_kernel(const T* __restrict__ src, T* __restrict__ dst, int H, int W, int C, int fw, int nearest) {
+  const int ow = 6 * fw;
+  const int pix = blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= fw * ow) return;
+  const int r = pix / ow, col = pix - r * ow;
+  const int face = col / fw, c = col - face * fw;
+  const float a = np_linspace_f32(-0.5, 0.5, fw, c), b = -np_linspace_f32(-0.5, 0.5, fw, r);
+  float x, y, z;
+  switch (face) {  // F R B L U D: the face's plane coordinate is +-0.5, the grid (a, b) spans the other two axes
+    case 0: x = a; y = b; z = 0.5f; break;
+    case 1: z = a; y = b; x = 0.5f; break;
+    case 2: x = a; y = b; z = -0.5f; break;
+    case 3: z = a; y = b; x = -0.5f; break;
+    case 4: x = a; z = b; y = 0.5f; break;
+    default: x = a; z = b; y = -0.5f; break;
+  }
+  const float u = f32_atan2(x, z);
+  const float v = f32_atan2(y, __fsqrt_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(z, z))));
+  const float cx = __fsub_rn(__fmul_rn(__fadd_rn(__fdiv_rn(u, float(2.0 * M_PI)), 0.5f), float(W)), 0.5f);
+  const float cy = __fsub_rn(__fmul_rn(__fadd_rn(__fdiv_rn(-v, float(M_PI)), 0.5f), float(H)), 0.5f);
+  py360_sample_equirec(src, H, W, C, double(cx), double(cy), nearest, dst + (size_t)pix * C);
+}
+
+// Pixel of the horizon cube behind sample (y, x) of padded face f of sample_cubefaces (utils.py:135-173), or -1 for
+// one of its zero pads. Inside the face: the R / B column flip and the U row flip. On the two pad rows / columns: the
+// host's border table, per face [row fw][fw], [row fw+1][fw], [col fw][fw+2], [col fw+1][fw+2].
+__device__ __forceinline__ int c2e_src(int f, int y, int x, int fw, const int* __restrict__ border) {
+  if (y < fw && x < fw) {
+    if (f == 1 || f == 2) x = fw - 1 - x;
+    if (f == 4) y = fw - 1 - y;
+    return y * 6 * fw + f * fw + x;
+  }
+  const int* bt = border + (size_t)f * (4 * fw + 4);
+  return __ldg(x < fw ? bt + (y - fw) * fw + x : bt + 2 * fw + (x - fw) * (fw + 2) + y);
+}
+
+template <typename T>
+__device__ __forceinline__ double c2e_tap(const T* __restrict__ cube, int idx, int C, int ch) {
+  return idx < 0 ? 0.0 : double(cube[(size_t)idx * C + ch]);
+}
+
+// c2e.py:6-64: thread <-> one equirect pixel, every channel. The face comes from the host's ceiling-row table
+// (equirect_facetype, utils.py:47-64), the face coordinates from float32 math as numpy evaluates it, the clip and
+// scale and the bilinear sum in float64 in scipy's term order ((v * wy) * wx, summed row-major) — the padded faces
+// are float64, so the result is too.
+template <typename T>
+__global__ void __launch_bounds__(256)
+c2e_py360_kernel(const T* __restrict__ cube, double* __restrict__ dst, int fw, int C, int h, int w,
+                 const int* __restrict__ ceil_rows, const int* __restrict__ border, int nearest) {
+  const int pix = blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= h * w) return;
+  const int i = pix / w, j = pix - i * w;
+  // face type: the four side faces rolled by 3w/8, ceiling rows [0, ceil) are U, their mirror image D
+  const int q4 = w / 4;
+  const int xs = (j - 3 * w / 8 + w) % w;
+  const int ceil_i = __ldg(ceil_rows + xs % q4);
+  int face = xs / q4;
+  if (i < ceil_i) face = 4;
+  if (h - 1 - i < ceil_i) face = 5;
+  // equirect_uvgrid: float32 linspace; v's halving is exact
+  const float u = np_linspace_f32(-M_PI, M_PI, w, j);
+  const float v = __fmul_rn(np_linspace_f32(M_PI, -M_PI, h, i), 0.5f);
+  float fx, fy;
+  if (face < 4) {
+    const float a = __fsub_rn(u, float(__dmul_rn(M_PI, double(face)) * 0.5));
+    fx = __fmul_rn(0.5f, f32_tan(a));
+    fy = __fdiv_rn(__fmul_rn(-0.5f, f32_tan(v)), f32_cos(a));
+  } else {
+    const float cc = __fmul_rn(0.5f, f32_tan(__fsub_rn(float(M_PI / 2), face == 4 ? v : fabsf(v))));
+    fx = __fmul_rn(cc, f32_sin(u));
+    fy = __fmul_rn(face == 4 ? cc : -cc, f32_cos(u));
+  }
+  // clip to the face and scale to [0, fw]: always inside the (fw + 2)-wide padded face, so the 'wrap' boundary
+  // never applies and the +1 neighbour is at most index fw + 1
+  const double X = __dmul_rn(__dadd_rn(fmin(fmax(double(fx), -0.5), 0.5), 0.5), double(fw));
+  const double Y = __dmul_rn(__dadd_rn(fmin(fmax(double(fy), -0.5), 0.5), 0.5), double(fw));
+  double* out = dst + (size_t)pix * C;
+  if (nearest) {
+    const int idx = c2e_src(face, int(floor(Y + 0.5)), int(floor(X + 0.5)), fw, border);
+    for (int ch = 0; ch < C; ++ch) out[ch] = c2e_tap(cube, idx, C, ch);
+    return;
+  }
+  const int y0 = int(floor(Y)), x0 = int(floor(X));
+  const double ty = Y - double(y0), tx = X - double(x0);
+  const int i00 = c2e_src(face, y0, x0, fw, border), i01 = c2e_src(face, y0, x0 + 1, fw, border);
+  const int i10 = c2e_src(face, y0 + 1, x0, fw, border), i11 = c2e_src(face, y0 + 1, x0 + 1, fw, border);
+  const double wy0 = 1.0 - ty, wx0 = 1.0 - tx;
+  for (int ch = 0; ch < C; ++ch) {
+    double acc = __dmul_rn(__dmul_rn(c2e_tap(cube, i00, C, ch), wy0), wx0);
+    acc = __dadd_rn(acc, __dmul_rn(__dmul_rn(c2e_tap(cube, i01, C, ch), wy0), tx));
+    acc = __dadd_rn(acc, __dmul_rn(__dmul_rn(c2e_tap(cube, i10, C, ch), ty), wx0));
+    out[ch] = __dadd_rn(acc, __dmul_rn(__dmul_rn(c2e_tap(cube, i11, C, ch), ty), tx));
+  }
+}
+
 }  // namespace pf
 
 extern "C" int pf_e2p_py360(const void* src, void* dst, int is_u8, int H, int W, int C, int h, int w, const double* cams,
@@ -500,6 +621,50 @@ extern "C" int pf_e2p_py360(const void* src, void* dst, int is_u8, int H, int W,
   else
     e2p_py360_kernel<float><<<grid, 256, 0, st>>>(static_cast<const float*>(src), static_cast<float*>(dst), H, W, C, h, w, cams, mode);
   PF_CHECK_LAUNCH("e2p_py360_kernel");
+  return PF_OK;
+}
+
+extern "C" int pf_c2e_py360(const void* cube, double* dst, int is_u8, int face_w, int C, int h, int w,
+                            const int* ceil_rows, const int* border, int mode, void* stream) {
+  using namespace pf;
+  PF_CHECK_ARG(cube && dst && ceil_rows && border, "pf_c2e_py360: null pointer");
+  PF_CHECK_ARG(face_w > 0 && C > 0 && h > 0 && w > 0, "pf_c2e_py360: empty shape");
+  // c2e.py:26 asserts w % 8 == 0: the face-type roll by 3w/8 and the w/4 ceiling table need it
+  PF_CHECK_ARG(w % 8 == 0, "pf_c2e_py360: w = %d must be a multiple of 8", w);
+  PF_CHECK_ARG((long long)h * w < (1LL << 31) && (long long)face_w * 6 * face_w < (1LL << 31),
+               "pf_c2e_py360: %d x %d panorama or face_w %d exceeds 2^31 pixels", h, w, face_w);
+  if (mode != 0 && mode != 1) {
+    set_error("pf_c2e_py360: unknown mode");
+    return PF_ERR_UNSUPPORTED;
+  }
+  const unsigned blocks = unsigned(((long long)h * w + 255) / 256);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (is_u8)
+    c2e_py360_kernel<uint8_t><<<blocks, 256, 0, st>>>(static_cast<const uint8_t*>(cube), dst, face_w, C, h, w, ceil_rows, border, mode);
+  else
+    c2e_py360_kernel<float><<<blocks, 256, 0, st>>>(static_cast<const float*>(cube), dst, face_w, C, h, w, ceil_rows, border, mode);
+  PF_CHECK_LAUNCH("c2e_py360_kernel");
+  return PF_OK;
+}
+
+extern "C" int pf_e2c_py360(const void* src, void* dst, int is_u8, int H, int W, int C, int face_w, int mode,
+                            void* stream) {
+  using namespace pf;
+  PF_CHECK_ARG(src && dst, "pf_e2c_py360: null pointer");
+  PF_CHECK_ARG(H > 1 && W > 1 && C > 0 && face_w > 0, "pf_e2c_py360: bad shape");
+  PF_CHECK_ARG((long long)face_w * 6 * face_w < (1LL << 31) && (long long)(H + 2) * W < (1LL << 31),
+               "pf_e2c_py360: face_w %d or %d x %d image exceeds 2^31 pixels", face_w, H, W);
+  if (mode != 0 && mode != 1) {
+    set_error("pf_e2c_py360: unknown mode");
+    return PF_ERR_UNSUPPORTED;
+  }
+  const unsigned blocks = unsigned(((long long)face_w * 6 * face_w + 255) / 256);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (is_u8)
+    e2c_py360_kernel<uint8_t><<<blocks, 256, 0, st>>>(static_cast<const uint8_t*>(src), static_cast<uint8_t*>(dst), H, W, C, face_w, mode);
+  else
+    e2c_py360_kernel<float><<<blocks, 256, 0, st>>>(static_cast<const float*>(src), static_cast<float*>(dst), H, W, C, face_w, mode);
+  PF_CHECK_LAUNCH("e2c_py360_kernel");
   return PF_OK;
 }
 
