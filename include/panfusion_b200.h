@@ -4,7 +4,8 @@
  * Every entry point takes plain device pointers, sizes and a CUDA stream (cudaStream_t passed as void*).
  * The caller (PyTorch on the host side) owns every buffer; the library keeps no hidden state except a
  * thread-local error string. All functions return 0 on success or a negative PF_ERR_* code; launches are
- * asynchronous on the given stream and CUDA-graph capturable (no allocation, no host sync inside).
+ * asynchronous on the given stream and CUDA-graph capturable (no allocation, no host sync inside), except
+ * pf_frechet_fp64, which reads its convergence test back once per Jacobi sweep.
  *
  * Each declaration cites the reference interface (file:line under the upstream repo) it replaces.
  * Tensors are row-major; "tokens" layout means [N*H*W, C] channels-last, "NCHW" is the reference's layout.
@@ -380,6 +381,36 @@ int pf_cpattn_attn(const void* q, int ldq, const void* kv, int ldkv, void* out, 
  * records (PF_CAM_DOUBLES each, device). */
 int pf_mp2e(const uint8_t* views, int m, int hp, int wp, int C, const double* cams_p2e, int He, int We, uint8_t* out,
             void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * FAED (models/faed/FAED.py:50-103, encoder models/faed/modules.py:5-36,176-264). Activations are channels-last fp16
+ * [B, H, W, C]; CircularPadding(p) (modules.py:5-19: rows zero-padded, columns wrapped, corners zero) is addressing
+ * inside pf_conv_circ, no padded copy.
+ * pf_faed_prep (FAED.py:70, Encoder.forward's x[:, :3], modules.py:249): src [B, C, H, W] uint8 (is_u8) or fp32, first
+ * 3 channels -> dst fp16 [B, H, W, 16] = src / 127.5 - 1 in fp32, rounded once; channels 3..15 are zero. */
+int pf_faed_prep(const void* src, int is_u8, int B, int C, int H, int W, void* dst, void* stream);
+/* Conv2d = CircularPadding(pad) + unpadded nn.Conv2d (modules.py:22-36) with BN folded into w/bias, then ReLU (relu != 0),
+ * then + residual (ResBlock, modules.py:59-65). x fp16 [B, H, W, Cin], w fp16 [k*k][Cin][Cout] (tap-major ky, kx), bias
+ * fp32 [Cout], residual fp16 [B, Ho, Wo, Cout] or NULL, out [B, Ho, Wo, Cout] fp16 or fp32 (out_dtype PF_F16 / PF_F32).
+ * Layers: k 3/5/7/9 stride 1 pad k/2, or k 4 stride 2 pad 1; Cin 16/32/64/128, Cout 32/64/128 (Cin >= 64 -> Cout 64/128,
+ * Cin 16 -> Cout 32); anything else is PF_ERR_UNSUPPORTED. */
+int pf_conv_circ(const void* x, int B, int H, int W, int Cin, const void* w, const float* bias, int Cout, int k,
+                 int stride, int pad, int relu, const void* residual, void* out, int out_dtype, void* stream);
+/* FAED.py:72-77: x fp32 [B, h, w, C] -> out fp32 [B, C*h], out[b, c*h + y] = weight[y] * mean_x x[b, y, x, c];
+ * weight [h] = cos(linspace(pi/2, -pi/2, h)) in fp32 (device). */
+int pf_faed_pool(const float* x, int B, int h, int w, int C, const float* weight, float* out, void* stream);
+/* FAED.py:80-90: sum[d] += sum_i X[i], cov_sum[d, d] += X^T X in fp64 for X fp32 [n, d]; every element is summed over i in
+ * order, so repeated calls give identical bits. */
+int pf_faed_stats(const float* features, int n, int d, double* sum, double* cov_sum, void* stream);
+/* FAED.py:92-103 + torchmetrics _compute_fid: out[0] = |mu1 - mu2|^2 + tr S1 + tr S2 - 2 sum sqrt(eig(S1 S2)) in fp64,
+ * S = (cov_sum - n mu mu^T) / (n - 1), mu = sum / n. The square-root term is the nuclear norm of L1^T L2 with
+ * S_i = L_i L_i^T, both from one-sided Jacobi iterations (negative rounding-level eigenvalues clamped to 0). ws: device,
+ * pf_frechet_ws_doubles(d) doubles; d % 64 == 0; n1, n2 >= 2. sweeps: host int[3] (or NULL) <- the sweeps of the
+ * Jacobi iterations on S1, S2 and L1^T L2. Synchronizes the stream once per Jacobi sweep; a Jacobi
+ * that does not converge in 100 sweeps returns PF_ERR_UNSUPPORTED. */
+long long pf_frechet_ws_doubles(int d);
+int pf_frechet_fp64(const double* sum1, const double* cov_sum1, long long n1, const double* sum2,
+                    const double* cov_sum2, long long n2, int d, double* ws, double* out, int* sweeps, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * View-sharded step (SURVEY.md 8e): device-initiated all-gather over NVLink peer mappings, capturable in a CUDA graph.

@@ -89,6 +89,7 @@ EXPORTS = [
     "pf_eppa_tables", "pf_eppa_pe", "pf_cpattn_tables", "pf_cpattn_gather", "pf_cpattn_attn", "pf_mp2e",
     "pf_allgather_views", "pf_enable_peer_access", "pf_comm_alloc", "pf_comm_free", "pf_ipc_export", "pf_ipc_open",
     "pf_ipc_close", "pf_embed_tokens", "pf_add_noise", "pf_mse_loss_ws_floats", "pf_mse_loss", "pf_gaussian_sample",
+    "pf_faed_prep", "pf_conv_circ", "pf_faed_pool", "pf_faed_stats", "pf_frechet_ws_doubles", "pf_frechet_fp64",
 ]
 
 
