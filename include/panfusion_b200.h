@@ -413,6 +413,46 @@ int pf_frechet_fp64(const double* sum1, const double* cov_sum1, long long n1, co
                     const double* cov_sum2, long long n2, int d, double* ws, double* out, int* sweeps, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * FID and Inception Score (models/pano/EvalPanoGen.py:30-49: torchmetrics FrechetInceptionDistance / InceptionScore over
+ * torch-fidelity's FeatureExtractorInceptionV3, the network of torchmetrics' NoTrainInceptionV3). Activations are
+ * channels-last fp16 [B, H, W, C]. FID's statistics and distance are pf_faed_stats and pf_frechet_fp64 at d = 2048.
+ * pf_inception_prep (FeatureExtractorInceptionV3.forward: x.float(), interpolate_bilinear_2d_like_tensorflow1x to
+ * 299x299 with align_corners=False, method 'slow', then (x - 128) / 128): src [B, 3, H, W] uint8 (is_u8 = 1) or fp32 in
+ * [0, 1] (is_u8 = 0: torchmetrics' normalize=True, (x * 255).byte() truncation applied per pixel) -> dst fp16
+ * [B, 299, 299, 16], channels 3..15 zero. Each op is one fp32 op, as torch runs it. */
+int pf_inception_prep(const void* src, int is_u8, int B, int H, int W, void* dst, void* stream);
+/* Width Cw of pf_conv2d_nhwc's packed weight and bias: Cout rounded up to 32 if Cout <= 32, else to a multiple of 64. */
+int pf_conv2d_packed_cout(int Cout);
+/* BasicConv2d (conv without bias + BatchNorm(eps 1e-3) + ReLU) with BN folded into w / bias: zero-padded kh x kw
+ * convolution (kh, kw <= 7, per-axis pad < k, stride 1 or 2, the same on both axes), then ReLU if relu != 0. The
+ * implicit-GEMM mma.sync core of pf_conv_circ. x fp16 [B, H, W, Cin] with Cin % 16 == 0; w fp16 [kh*kw][Cin][Cw]
+ * (tap-major ky, kx; zero columns past Cout); bias fp32 [Cw]. out fp16 or fp32 (out_dtype) [B, Ho, Wo, out_ld] of which
+ * channels [out_off, out_off + Cout) are written and the rest left untouched: a branch writes its slice of the
+ * concat buffer. Cout, out_ld and out_off even. */
+int pf_conv2d_nhwc(const void* x, int B, int H, int W, int Cin, const void* w, const float* bias, int Cout, int kh,
+                   int kw, int stride, int ph, int pw, int relu, void* out, int out_dtype, int out_ld, int out_off,
+                   void* stream);
+/* 3x3 pools of the FID InceptionV3 on fp16 [B, H, W, C] (C % 8 == 0) -> out [B, Ho, Wo, out_ld] channels
+ * [out_off, out_off + C) (multiples of 8). PF_POOL_MAX: F.max_pool2d (stem, Mixed_6a / 7a with stride 2 pad 0; Mixed_7c's
+ * pool branch with stride 1 pad 1). PF_POOL_AVG_EXCL_PAD: F.avg_pool2d(count_include_pad=False), fp32 sum in tap order,
+ * rounded once (Mixed_5b..7b's pool branch, stride 1 pad 1). */
+#define PF_POOL_MAX 0
+#define PF_POOL_AVG_EXCL_PAD 1
+int pf_pool2d_nhwc(const void* x, int B, int H, int W, int C, int mode, int stride, int pad, void* out, int out_ld,
+                   int out_off, void* stream);
+/* FeatureExtractorInceptionV3's head: x fp32 [B, HW, C] (Mixed_7c, HW = 8x8) -> pool3 fp32 [B, C] (the mean over HW,
+ * adaptive_avg_pool2d) and logits fp32 [B, N] = pool3 @ fc_w^T with fc_w fp32 [N, C] ('logits_unbiased': no bias).
+ * Every output is summed in a fixed order, independent of B. */
+int pf_inception_head(const float* x, int B, int HW, int C, const float* fc_w, int N, float* pool3, float* logits,
+                      void* stream);
+/* torchmetrics InceptionScore.compute after its randperm: logits fp32 [n, C], perm int64 [n] (device) -> out fp32 [2] =
+ * (mean, unbiased std) over the torch.chunk(splits) chunks (ceil(n / splits) rows each) of exp(mean KL(p || chunk mean
+ * p)), computed in fp64; one chunk gives std = nan. ws: device, pf_inception_score_ws_doubles(n, C, splits) doubles. */
+long long pf_inception_score_ws_doubles(int n, int C, int splits);
+int pf_inception_score(const float* logits, const long long* perm, int n, int C, int splits, double* ws, float* out,
+                       void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * View-sharded step (SURVEY.md 8e): device-initiated all-gather over NVLink peer mappings, capturable in a CUDA graph.
  * The reference has no model parallelism (Lightning DDP over prompts, main.py:63); this is the exchange the view partition
  * needs: models/pano/modules.py:44-48 lets every panorama query attend to the keys / values of ALL views, so each rank

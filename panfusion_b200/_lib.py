@@ -90,6 +90,8 @@ EXPORTS = [
     "pf_allgather_views", "pf_enable_peer_access", "pf_comm_alloc", "pf_comm_free", "pf_ipc_export", "pf_ipc_open",
     "pf_ipc_close", "pf_embed_tokens", "pf_add_noise", "pf_mse_loss_ws_floats", "pf_mse_loss", "pf_gaussian_sample",
     "pf_faed_prep", "pf_conv_circ", "pf_faed_pool", "pf_faed_stats", "pf_frechet_ws_doubles", "pf_frechet_fp64",
+    "pf_inception_prep", "pf_conv2d_packed_cout", "pf_conv2d_nhwc", "pf_pool2d_nhwc", "pf_inception_head",
+    "pf_inception_score_ws_doubles", "pf_inception_score",
 ]
 
 

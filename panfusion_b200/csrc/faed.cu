@@ -4,16 +4,14 @@
 //
 // Activations are channels-last fp16 [B, H, W, C]. CircularPadding(p) zero-pads rows and wraps columns (corners are
 // zero), so the convolution addresses its operand directly: input row iy = oy*s + ky - p is zero outside [0, H), input
-// column ix = ox*s + kx - p is taken modulo W. No padded copy is made.
-#include "pf_common.cuh"
+// column ix = ox*s + kx - p is taken modulo W. No padded copy is made. pf_conv_circ runs the implicit-GEMM core of
+// conv_mma.cuh (shared with the FID InceptionV3) with circular padding.
+#include "conv_mma.cuh"
 
 namespace pf {
 namespace faed {
 
-constexpr int kPrepC = 16;   // the first layer's operand: 3 image channels + 13 zero channels (one 16-wide MMA k-step)
-constexpr int kBM = 128;     // output pixels per CTA
-constexpr int kThreads = 256;
-constexpr int kStages = 3;
+constexpr int kPrepC = 16;  // the first layer's operand: 3 image channels + 13 zero channels (one 16-wide MMA k-step)
 
 // ---------------------------------------------------------------------------------------------------------------------
 // pf_faed_prep: x = img.float32 / 127.5 - 1 (FAED.py:70), rounded once to fp16, NCHW -> [B, H, W, 16]
@@ -36,200 +34,6 @@ prep_kernel(const void* __restrict__ src, int is_u8, int B, int C, int H, int W,
   uint4* d = reinterpret_cast<uint4*>(dst + idx * kPrepC);
   d[0] = reinterpret_cast<const uint4*>(v)[0];
   d[1] = reinterpret_cast<const uint4*>(v)[1];
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// pf_conv_circ: implicit-GEMM convolution on mma.sync m16n8k16 (fp16 in, fp32 accumulate).
-// GEMM view: M = B*Ho*Wo output pixels, N = Cout, K = k*k taps x Cin. A k-step is one tap x KC input channels, so a
-// 32-channel layer runs 32-wide k-steps and a 32-wide N tile: nothing is zero-padded to 64.
-// CTA: 128 pixels x Cout, 8 warps as 4 (M, 32 rows) x 2 (N, Cout/2 columns); 3-stage cp.async ring; the A rows are
-// gathered per pixel (16-byte pieces, zero-filled for rows outside the image) and the B rows are the packed weight
-// [tap][Cin][Cout]. Shared rows are padded by 16 bytes so the ldmatrix phases hit distinct banks.
-// ---------------------------------------------------------------------------------------------------------------------
-struct ConvArgs {
-  const __half* x;
-  const __half* w;
-  const float* bias;
-  const __half* residual;
-  void* out;
-  int B, H, W, Cin, Cout, Ho, Wo, k, stride, pad, relu, out_f32;
-  int M;
-};
-
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void mma16816(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-template <int KC, int BN>
-struct ConvTile {
-  static constexpr int A_LD = KC + 8, B_LD = BN + 8;  // halves
-  static constexpr int A_HALVES = kBM * A_LD, B_HALVES = KC * B_LD;
-  static constexpr int STAGE_HALVES = A_HALVES + B_HALVES;
-  static constexpr int SMEM = kStages * STAGE_HALVES * 2;
-  static constexpr int CPR = KC / 8;                    // 16-byte pieces per A row
-  static constexpr int A_ITERS = kBM * CPR / kThreads;  // pieces per thread
-  static constexpr int NT = BN / 16;                    // n8 tiles per warp
-};
-
-template <int KC, int BN>
-__global__ void __launch_bounds__(kThreads)
-conv_circ_kernel(ConvArgs a) {
-  using T = ConvTile<KC, BN>;
-  static_assert(T::A_ITERS >= 1 && T::NT % 2 == 0, "tile");
-  extern __shared__ __align__(16) __half smem[];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int wm = warp & 3, wn = warp >> 2;
-  const int m0 = blockIdx.x * kBM;
-  const int HoWo = a.Ho * a.Wo;
-
-  // per-thread A pieces: the pixel's image offset and its top-left input coordinate
-  int a_base[T::A_ITERS], a_y[T::A_ITERS], a_x[T::A_ITERS], a_dst[T::A_ITERS];
-#pragma unroll
-  for (int i = 0; i < T::A_ITERS; ++i) {
-    const int idx = tid + i * kThreads, row = idx / T::CPR, ch = idx % T::CPR;
-    const int m = m0 + row;
-    a_dst[i] = row * T::A_LD + ch * 8;
-    if (m < a.M) {
-      const int b = m / HoWo, r = m % HoWo;
-      a_base[i] = b * a.H;
-      a_y[i] = (r / a.Wo) * a.stride - a.pad;
-      a_x[i] = (r % a.Wo) * a.stride - a.pad;
-    } else {
-      a_base[i] = 0;
-      a_y[i] = -(1 << 20);  // never inside the image: zero-filled
-      a_x[i] = 0;
-    }
-  }
-  const int chunks = a.Cin / KC;
-  const int steps = a.k * a.k * chunks;
-
-  auto load = [&](int s, int buf) {
-    __half* As = smem + buf * T::STAGE_HALVES;
-    __half* Bs = As + T::A_HALVES;
-    const int tap = s / chunks, c0 = (s % chunks) * KC;
-    const int ky = tap / a.k, kx = tap % a.k;
-#pragma unroll
-    for (int i = 0; i < T::A_ITERS; ++i) {
-      const int ch = (tid + i * kThreads) % T::CPR;
-      const int iy = a_y[i] + ky;
-      int ix = a_x[i] + kx;
-      ix = ix < 0 ? ix + a.W : (ix >= a.W ? ix - a.W : ix);
-      const bool valid = iy >= 0 && iy < a.H;
-      const __half* src = valid ? a.x + ((size_t)(a_base[i] + iy) * a.W + ix) * a.Cin + c0 + ch * 8 : a.x;
-      cp_async16(smem_u32(As + a_dst[i]), src, valid);
-    }
-    const __half* wsrc = a.w + ((size_t)tap * a.Cin + c0) * a.Cout;
-    for (int idx = tid; idx < KC * BN / 8; idx += kThreads) {
-      const int r = idx / (BN / 8), c = idx % (BN / 8);
-      cp_async16(smem_u32(Bs + r * T::B_LD + c * 8), wsrc + (size_t)r * a.Cout + c * 8, true);
-    }
-  };
-
-  float acc[2][T::NT][4];
-#pragma unroll
-  for (int i = 0; i < 2; ++i)
-#pragma unroll
-    for (int j = 0; j < T::NT; ++j)
-#pragma unroll
-      for (int q = 0; q < 4; ++q) acc[i][j][q] = 0.f;
-
-#pragma unroll
-  for (int s = 0; s < kStages - 1; ++s) {
-    if (s < steps) load(s, s);
-    cp_async_commit();
-  }
-  for (int s = 0; s < steps; ++s) {
-    cp_async_wait<kStages - 2>();
-    __syncthreads();  // stage s landed for every thread; stage s-1's buffer is free
-    if (s + kStages - 1 < steps) load(s + kStages - 1, (s + kStages - 1) % kStages);
-    cp_async_commit();
-    const __half* As = smem + (s % kStages) * T::STAGE_HALVES;
-    const __half* Bs = As + T::A_HALVES;
-#pragma unroll
-    for (int kk = 0; kk < KC; kk += 16) {
-      uint32_t af[2][4];
-#pragma unroll
-      for (int mt = 0; mt < 2; ++mt) {
-        const int row = wm * 32 + mt * 16 + (lane & 15), col = kk + (lane >> 4) * 8;
-        ldsm_x4(smem_u32(As + row * T::A_LD + col), af[mt][0], af[mt][1], af[mt][2], af[mt][3]);
-      }
-#pragma unroll
-      for (int np = 0; np < T::NT / 2; ++np) {
-        uint32_t b0, b1, b2, b3;
-        const int krow = kk + (lane & 15), col = wn * (BN / 2) + np * 16 + (lane >> 4) * 8;
-        ldsm_x4_t(smem_u32(Bs + krow * T::B_LD + col), b0, b1, b2, b3);
-#pragma unroll
-        for (int mt = 0; mt < 2; ++mt) {
-          mma16816(acc[mt][2 * np], af[mt], b0, b1);
-          mma16816(acc[mt][2 * np + 1], af[mt], b2, b3);
-        }
-      }
-    }
-  }
-  cp_async_wait<0>();
-
-  // epilogue: + bias (BN folded), ReLU, + residual, 16-bit or fp32 store
-#pragma unroll
-  for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-    for (int nt = 0; nt < T::NT; ++nt) {
-      const int col = wn * (BN / 2) + nt * 8 + (lane & 3) * 2;
-      const float bias0 = a.bias[col], bias1 = a.bias[col + 1];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int m = m0 + wm * 32 + mt * 16 + (lane >> 2) + h * 8;
-        if (m >= a.M) continue;
-        float v0 = acc[mt][nt][2 * h] + bias0, v1 = acc[mt][nt][2 * h + 1] + bias1;
-        if (a.relu) {
-          v0 = fmaxf(v0, 0.f);
-          v1 = fmaxf(v1, 0.f);
-        }
-        const size_t o = (size_t)m * a.Cout + col;
-        if (a.residual) {
-          const float2 r = __half22float2(*reinterpret_cast<const __half2*>(a.residual + o));
-          v0 += r.x;
-          v1 += r.y;
-        }
-        if (a.out_f32)
-          *reinterpret_cast<float2*>(static_cast<float*>(a.out) + o) = make_float2(v0, v1);
-        else
-          *reinterpret_cast<__half2*>(static_cast<__half*>(a.out) + o) = __floats2half2_rn(v0, v1);
-      }
-    }
-}
-
-template <int KC, int BN>
-int launch_conv(const ConvArgs& a, cudaStream_t st) {
-  using T = ConvTile<KC, BN>;
-  static bool attr_set = false;  // per-kernel opt-in to > 48 KB of dynamic shared memory
-  if (!attr_set) {
-    const int rc = check_cuda(
-        cudaFuncSetAttribute(conv_circ_kernel<KC, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SMEM),
-        "cudaFuncSetAttribute(conv_circ_kernel)");
-    if (rc) return rc;
-    attr_set = true;
-  }
-  conv_circ_kernel<KC, BN><<<(unsigned)((a.M + kBM - 1) / kBM), kThreads, T::SMEM, st>>>(a);
-  PF_CHECK_LAUNCH("conv_circ_kernel");
-  return PF_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -499,6 +303,8 @@ int jacobi(double* A, double* V, int n, double* fro2, unsigned long long* off_de
 
 using namespace pf;
 using namespace pf::faed;
+using pf::convmma::ConvArgs;
+using pf::convmma::launch_conv;
 
 extern "C" int pf_faed_prep(const void* src, int is_u8, int B, int C, int H, int W, void* dst, void* stream) {
   PF_CHECK_ARG(src && dst, "pf_faed_prep: null pointer");
@@ -530,20 +336,21 @@ extern "C" int pf_conv_circ(const void* x, int B, int H, int W, int Cin, const v
   }
   PF_CHECK_ARG(pad < W, "pf_conv_circ: circular padding %d needs W > pad (W=%d)", pad, W);
   PF_CHECK_ARG(!(s2 && (H % 2 || W % 2)), "pf_conv_circ: the stride-2 layer needs even H and W (H=%d W=%d)", H, W);
+  // one N tile of width Cout (grid.y = 1), circular W; the weight is packed [k*k][Cin][Cout]
   ConvArgs a{static_cast<const __half*>(x), static_cast<const __half*>(w), bias,
              static_cast<const __half*>(residual), out, B, H, W, Cin, Cout,
-             (H + 2 * pad - k) / stride + 1, (W + 2 * pad - k) / stride + 1, k, stride, pad, relu,
-             out_dtype == PF_F32, 0};
+             (H + 2 * pad - k) / stride + 1, (W + 2 * pad - k) / stride + 1, k, k, stride, pad, pad, relu,
+             out_dtype == PF_F32, Cout, Cout, 0, 0};
   const long long M = (long long)B * a.Ho * a.Wo;
   PF_CHECK_ARG(M > 0 && M * (Cout > Cin ? Cout : Cin) < (1LL << 31), "pf_conv_circ: tensor too large");
   a.M = (int)M;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int kc = Cin >= 64 ? 64 : Cin;
-  if (kc == 16 && Cout == 32) return launch_conv<16, 32>(a, st);
-  if (kc == 32 && Cout == 32) return launch_conv<32, 32>(a, st);
-  if (kc == 32 && Cout == 64) return launch_conv<32, 64>(a, st);
-  if (kc == 64 && Cout == 64) return launch_conv<64, 64>(a, st);
-  if (kc == 64 && Cout == 128) return launch_conv<64, 128>(a, st);
+  if (kc == 16 && Cout == 32) return launch_conv<16, 32, true>(a, st);
+  if (kc == 32 && Cout == 32) return launch_conv<32, 32, true>(a, st);
+  if (kc == 32 && Cout == 64) return launch_conv<32, 64, true>(a, st);
+  if (kc == 64 && Cout == 64) return launch_conv<64, 64, true>(a, st);
+  if (kc == 64 && Cout == 128) return launch_conv<64, 128, true>(a, st);
   set_error("pf_conv_circ: Cin=%d -> Cout=%d is not a FAED encoder layer", Cin, Cout);
   return PF_ERR_UNSUPPORTED;
 }
