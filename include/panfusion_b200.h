@@ -109,6 +109,8 @@ int pf_p2e(const void* src, void* dst, uint8_t* mask, int dtype, int B, int C, i
  * act: PF_ACT_GEGLU expects B (and bias) packed so that every block_n-wide column tile holds block_n/2 value
  * columns followed by their block_n/2 gate columns; it writes N/2 output columns.
  * Constraints: Kc % 64 == 0, N % block_n == 0, block_n in {64,128,160,256}, a_ld/b_ld % 8 == 0.
+ * Alignment (checked, PF_ERR_INVALID otherwise): A, B, out, residual, rowbias, splitk_ws and ln_stats 16 bytes;
+ * row_stats_out 8 bytes; out_ld, res_ld % 8 == 0 and rowbias_ld % 4 == 0 (elements), so every row stays aligned.
  * ------------------------------------------------------------------------------------------------ */
 enum { PF_ACT_NONE = 0, PF_ACT_SILU = 1, PF_ACT_GELU = 2, PF_ACT_GEGLU = 3 };
 #define PF_MAX_TAPS 16

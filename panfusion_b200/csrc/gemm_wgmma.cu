@@ -571,6 +571,13 @@ extern "C" int pf_gemm_taps(const pf_gemm_args* a, void* stream) {
   PF_CHECK_ARG((reinterpret_cast<uintptr_t>(a->A) & 15) == 0 && (reinterpret_cast<uintptr_t>(a->B) & 15) == 0 &&
                    (reinterpret_cast<uintptr_t>(a->out) & 15) == 0,
                "pf_gemm_taps: operands must be 16-byte aligned");
+  // the epilogues and the split-K reduce read / write these with 16-byte (row statistics: 8-byte) vector accesses
+  PF_CHECK_ARG((reinterpret_cast<uintptr_t>(a->residual) & 15) == 0, "pf_gemm_taps: residual must be 16-byte aligned");
+  PF_CHECK_ARG(!a->rowbias || ((reinterpret_cast<uintptr_t>(a->rowbias) & 15) == 0 && a->rowbias_ld % 4 == 0),
+               "pf_gemm_taps: rowbias must be 16-byte aligned with rowbias_ld %% 4 == 0 (rowbias_ld=%d)", a->rowbias_ld);
+  PF_CHECK_ARG((reinterpret_cast<uintptr_t>(a->splitk_ws) & 15) == 0, "pf_gemm_taps: splitk_ws must be 16-byte aligned");
+  PF_CHECK_ARG((reinterpret_cast<uintptr_t>(a->row_stats_out) & 7) == 0,
+               "pf_gemm_taps: row_stats_out must be 8-byte aligned");
   PF_CHECK_ARG(a->out_dtype == PF_F32 || a->out_dtype == a->dtype, "pf_gemm_taps: out_dtype must be f32 or dtype");
   PF_CHECK_ARG(!a->residual || a->res_dtype == PF_F32 || a->res_dtype == a->dtype,
                "pf_gemm_taps: res_dtype must be f32 or dtype");
@@ -641,8 +648,7 @@ extern "C" int pf_gemm_taps(const pf_gemm_args* a, void* stream) {
     PF_CHECK_ARG(!a->ln_stats || (a->ln_colsum && a->ln_slots > 0 && a->ln_slots % 2 == 0 && a->ln_eps > 0.f &&
                                   (reinterpret_cast<uintptr_t>(a->ln_stats) & 15) == 0),
                  "pf_gemm_taps: ln_stats needs ln_colsum, ln_slots and ln_eps");
-    const bool plain16 = a->map_mode == 0 && a->out_dtype == a->dtype && (!a->residual || a->res_dtype == a->dtype) &&
-                         (reinterpret_cast<uintptr_t>(a->residual) & 15) == 0;
+    const bool plain16 = a->map_mode == 0 && a->out_dtype == a->dtype && (!a->residual || a->res_dtype == a->dtype);
     PF_CHECK_ARG(a->act == PF_ACT_GEGLU ? !a->row_stats_out : plain16,
                  "pf_gemm_taps: fused LayerNorm needs the plain row map with 16-bit output (consumer: or GEGLU)");
   }
@@ -664,8 +670,7 @@ extern "C" int pf_gemm_taps(const pf_gemm_args* a, void* stream) {
   }
   // staged TMA-store epilogue: plain row map, 16-bit output, 16-bit (or no) residual, no GEGLU
   const bool epi_tma = a->map_mode == 0 && a->out_dtype == a->dtype && a->act != PF_ACT_GEGLU &&
-                       (!a->residual || a->res_dtype == a->dtype) && bn != 256 &&
-                       (reinterpret_cast<uintptr_t>(a->residual) & 15) == 0;
+                       (!a->residual || a->res_dtype == a->dtype) && bn != 256;
   if (epi_tma) {
     switch (bn) {
       case 64: return launch_gemm<64, 8, true>(a, kp, st);

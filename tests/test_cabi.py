@@ -41,6 +41,31 @@ def test_bad_arguments_fail_loudly_without_gpu():
     assert lib.pf_gemm_pick_block_n(100, 0) == 0
 
 
+@pytest.mark.parametrize("field,value,extra,operand", [
+    ("residual", 0x40008, dict(res_ld=320, res_dtype=1), b"residual"),
+    ("rowbias", 0x40004, dict(rowbias_ld=320, rows_per_group=64), b"rowbias"),
+    ("rowbias", 0x40000, dict(rowbias_ld=322, rows_per_group=64), b"rowbias"),
+    ("splitk_ws", 0x40008, dict(k_splits=2), b"splitk_ws"),
+    ("row_stats_out", 0x40004, {}, b"row_stats_out"),
+])
+def test_misaligned_epilogue_operands_are_rejected_without_gpu(field, value, extra, operand):
+    """The epilogues and the split-K reduce access residual, rowbias and splitk_ws 16 bytes and row_stats_out 8 bytes at a
+    time: pf_gemm_taps refuses a misaligned one (or a rowbias row stride that misaligns its rows) before any CUDA call,
+    naming the operand. The pointers are never dereferenced."""
+    import ctypes as C
+    from panfusion_b200 import _lib
+    lib = _lib.lib()
+    a = _lib.GemmArgs()
+    a.A, a.a_rows, a.a_ld, a.B, a.b_ld, a.dtype = 0x10000, 512, 320, 0x20000, 320, 1
+    a.M, a.N, a.Kc, a.num_taps = 512, 320, 320, 1
+    a.out, a.out_ld, a.out_dtype = 0x30000, 320, 1
+    setattr(a, field, value)
+    for k, v in extra.items():
+        setattr(a, k, v)
+    rc = lib.pf_gemm_taps(C.byref(a), None)
+    assert rc == -1 and operand in lib.pf_last_error(), lib.pf_last_error()
+
+
 def test_no_cpu_path():
     from panfusion_b200 import geometry
     with pytest.raises(Exception):
