@@ -5,12 +5,20 @@
 // same channels-last image shifted by a constant row offset (zero-haloed "padded-flat" layout), so the im2col
 // matrix is never formed: each K-slab is one plain 2-D TMA box.
 //
-// Warp roles (288 threads): warps 0..3 and 4..7 = two consumer warpgroups, each owning 64 of the 128 tile rows
-// through the main loop; warp 8 = TMA producer (one lane). After the last K-slab the accumulators are written to
-// shared memory (over the now idle operand ring) and all 256 consumer threads run the epilogue with two threads per
-// tile row (even / odd 16-column chunks): bias / LayerNorm fold / per-image row bias / SiLU / GELU / GEGLU / residual,
-// then either (EPI_TMA) a swizzled staging tile written with TMA tile stores, or direct stores through the
-// halo-dropping row map (convolutions, fp32 outputs, GEGLU), or raw fp32 split-K partials.
+// 256 threads: warps 0..3 and 4..7 = two warpgroups, each owning 64 of the 128 tile rows through the main loop.
+// There is no producer warp: thread 0 fills the ring before the loop, and the leader of whichever warpgroup releases
+// a slot last issues the slot's next TMA loads, so no MMA-issuing warp ever blocks on the other warpgroup. After the last K-slab the accumulators are written to shared memory (over the now idle operand
+// ring) and all 256 threads run the epilogue with two threads per tile row (even / odd 16-column chunks): bias / LayerNorm fold / per-image row bias / SiLU / GELU / GEGLU / residual,
+// then either (EPI_TMA) swizzled [128][32] sub-tiles streamed out with TMA tile stores through two staging buffers
+// behind the accumulators, or direct stores through the halo-dropping row map (convolutions, fp32 outputs, GEGLU),
+// or raw fp32 split-K partials.
+//
+// Instantiations with a short ring (CTAS = 2) run TWO CTAs per SM (at most 128 registers per thread and 113 KB of
+// shared memory per CTA): a tile has no overlap of its own between ring fill, main loop, accumulator dump and
+// epilogue, so the tensor pipe is kept busy by the other CTA's main loop while one CTA fills or drains. A ninth
+// (producer) warp would rule that out: registers are granted to whole warps, nine warps would leave two CTAs 96
+// registers per thread, and the 160-wide tile alone holds 80 accumulators. The 256-wide GEGLU tile (128 accumulators,
+// 133 KB accumulator dump) and split-K, which is planned at about one CTA per SM, keep a long ring and CTAS = 1.
 #include <stdlib.h>
 
 #include "gemm_common.cuh"
@@ -18,32 +26,37 @@
 
 namespace pf {
 
-constexpr int GEMM_THREADS = 288;
-constexpr int GEMM_CONSUMERS = 256;
+constexpr int GEMM_THREADS = 256;
+
+constexpr int GEMM_SUB_BYTES = GEMM_BLOCK_M * 64;  // one [128][32] 16-bit sub-tile of the TMA-store epilogue, SWIZZLE_64B
+// an SM has 228 KB of shared memory and every resident CTA reserves 1 KB of it
+constexpr int GEMM_SMEM_CORESIDENT = 228 * 1024 / 2 - 1024;
 
 __host__ __device__ constexpr int gemm_acc_ld(int block_n) { return block_n + 4; }  // floats; +4: conflict-free rows
-__host__ __device__ constexpr int gemm_ring_bytes(int block_n, int stages) {
-  return ((stages * gemm_stage_bytes(block_n) > GEMM_BLOCK_M * gemm_acc_ld(block_n) * 4
-               ? stages * gemm_stage_bytes(block_n)
-               : GEMM_BLOCK_M * gemm_acc_ld(block_n) * 4) + 1023) / 1024 * 1024;
+// accumulator dump, rounded up to the 1024 bytes that keep the staging buffers behind it swizzle-aligned
+__host__ __device__ constexpr int gemm_acc_bytes(int block_n) {
+  return (GEMM_BLOCK_M * gemm_acc_ld(block_n) * 4 + 1023) / 1024 * 1024;
 }
-// full + empty barrier per stage and the residual barrier, 8 bytes each, rounded up to keep s_bias 16-byte aligned
-__host__ __device__ constexpr int gemm_bar_bytes(int stages) { return ((2 * stages + 1) * 8 + 15) / 16 * 16; }
+// the operand ring; after the main loop the same bytes hold the accumulators and (EPI_TMA) two staging sub-tiles
+__host__ __device__ constexpr int gemm_ring_bytes(int block_n, int stages, bool epi_tma) {
+  const int ring = stages * gemm_stage_bytes(block_n);
+  const int epi = gemm_acc_bytes(block_n) + (epi_tma ? 2 * GEMM_SUB_BYTES : 0);
+  return ((ring > epi ? ring : epi) + 1023) / 1024 * 1024;
+}
+// full barrier (8 bytes) and release counter (4 bytes) per stage, rounded up to keep s_bias 16-byte aligned
+__host__ __device__ constexpr int gemm_bar_bytes(int stages) { return (stages * 12 + 15) / 16 * 16; }
 __host__ __device__ constexpr int gemm_smem_bytes(int block_n, int stages, bool epi_tma) {
-  return gemm_ring_bytes(block_n, stages) + (epi_tma ? GEMM_BLOCK_M * block_n * 2 : 0) + gemm_bar_bytes(stages) +
+  return gemm_ring_bytes(block_n, stages, epi_tma) + gemm_bar_bytes(stages) +
          2 * block_n * 4 /*bias row + LayerNorm column sums*/;
 }
 
-template <int BLOCK_N, int STAGES, bool BF16, bool EPI_TMA>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
+template <int BLOCK_N, int STAGES, int CTAS, bool BF16, bool EPI_TMA>
+__global__ void __launch_bounds__(GEMM_THREADS, CTAS)
 gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR,
-                 const GemmKernelParams p) {
+                 const __grid_constant__ CUtensorMap tmC, const GemmKernelParams p) {
   constexpr int A_BYTES = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;
   constexpr int STAGE_BYTES = gemm_stage_bytes(BLOCK_N);
-  constexpr int RING_BYTES = gemm_ring_bytes(BLOCK_N, STAGES);
-  constexpr int STAGING_BYTES = EPI_TMA ? GEMM_BLOCK_M * BLOCK_N * 2 : 0;
-  constexpr int SUB_BYTES = GEMM_BLOCK_M * 64;  // one [128][32] 16-bit sub-tile, SWIZZLE_64B
+  constexpr int RING_BYTES = gemm_ring_bytes(BLOCK_N, STAGES, EPI_TMA);
   constexpr int ACC_LD = gemm_acc_ld(BLOCK_N);
   constexpr int NCH = BLOCK_N / 16;
   constexpr int NACC = BLOCK_N / 2;  // fp32 accumulators per thread of an m64 x BLOCK_N warpgroup tile
@@ -53,15 +66,15 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   float* sacc = reinterpret_cast<float*>(smem);  // [128][ACC_LD] fp32, over the ring once the main loop is done
-  uint8_t* staging = smem + RING_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + STAGING_BYTES);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* res_full_bar = empty_bar + STAGES;
-  float* s_bias = reinterpret_cast<float*>(staging + STAGING_BYTES + gemm_bar_bytes(STAGES));  // [BLOCK_N]
+  uint8_t* staging = smem + gemm_acc_bytes(BLOCK_N);  // EPI_TMA: two [128][32] 16-bit sub-tiles, also inside the ring
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + RING_BYTES);
+  uint32_t* released = reinterpret_cast<uint32_t*>(full_bar + STAGES);  // per slot: releases by the two warpgroups
+  float* s_bias = reinterpret_cast<float*>(smem + RING_BYTES + gemm_bar_bytes(STAGES));  // [BLOCK_N]
   float* s_cs = s_bias + BLOCK_N;                                            // [BLOCK_N] LayerNorm column sums
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int et = threadIdx.x;  // 0..255
+  const int lane = et & 31;
+  const int wg = et >> 7;  // warpgroup: tile rows [64 wg, 64 wg + 64)
   const int n_tiles = p.N / BLOCK_N;
   const int n_tile = int(blockIdx.x) % n_tiles;  // n fastest: concurrent CTAs share the A tile through L2
   const int m0 = (int(blockIdx.x) / n_tiles) * GEMM_BLOCK_M;
@@ -71,48 +84,33 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int kb_begin = (p.k_splits > 1) ? (int)((long long)split * p.num_kb / p.k_splits) : 0;
   const int kb_end = (p.k_splits > 1) ? (int)((long long)(split + 1) * p.num_kb / p.k_splits) : p.num_kb;
 
-  if (warp == 8 && lane == 0) {
+  if (et == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);  // one arrival per consumer warpgroup
+      released[s] = 0u;
     }
-    mbar_init(res_full_bar, 1);
     if constexpr (EPI_TMA) tma_prefetch_desc(&tmC);
     fence_barrier_init();
   }
   __syncthreads();
 
-  if (warp == 8) {
-    // ------------------------------ TMA producer ------------------------------
-    if (lane == 0) {
-      if constexpr (EPI_TMA) {
-        if (p.residual) {
-          mbar_expect_tx(res_full_bar, STAGING_BYTES);
-#pragma unroll
-          for (int sub = 0; sub < BLOCK_N / 32; ++sub)
-            tma_load_2d(staging + sub * SUB_BYTES, &tmR, res_full_bar, n0 + sub * 32, m0);
-        }
-      }
-      for (int kb = kb_begin; kb < kb_end; ++kb) {
-        const int s = (kb - kb_begin) % STAGES;
-        const uint32_t ph = ((kb - kb_begin) / STAGES) & 1;
-        mbar_wait(&empty_bar[s], ph ^ 1);
-        const int tap = kb / p.kb_per_tap;
-        const int kk = kb - tap * p.kb_per_tap;
-        uint8_t* sa = smem + s * STAGE_BYTES;
-        mbar_expect_tx(&full_bar[s], STAGE_BYTES);
-        tma_load_2d(sa, &tmA, &full_bar[s], kk * GEMM_BLOCK_K, m0 + p.tap_off[tap]);
-        tma_load_2d(sa + A_BYTES, &tmB, &full_bar[s], kb * GEMM_BLOCK_K, n0);
-      }
-    }
-    return;  // the producer takes no part in the epilogue's named barriers
+  // one K-slab into its ring slot (one thread): the A box of the slab's tap and the B box of the slab
+  auto load_slab = [&](int kb) {
+    const int s = (kb - kb_begin) % STAGES;
+    const int tap = kb / p.kb_per_tap;
+    const int kk = kb - tap * p.kb_per_tap;
+    uint8_t* sa = smem + s * STAGE_BYTES;
+    mbar_expect_tx(&full_bar[s], STAGE_BYTES);
+    tma_load_2d(sa, &tmA, &full_bar[s], kk * GEMM_BLOCK_K, m0 + p.tap_off[tap]);
+    tma_load_2d(sa + A_BYTES, &tmB, &full_bar[s], kb * GEMM_BLOCK_K, n0);
+  };
+  if (et == 0) {
+    for (int kb = kb_begin; kb < kb_end && kb < kb_begin + STAGES; ++kb) load_slab(kb);
   }
 
-  // ------------------------------ consumers: main loop ------------------------------
-  const int et = threadIdx.x;  // 0..255
-  const int wg = et >> 7;      // warpgroup: tile rows [64 wg, 64 wg + 64)
+  // ------------------------------ main loop ------------------------------
   if (p.bias && et < BLOCK_N) s_bias[et] = __ldg(p.bias + n0 + et);
   if (p.ln_stats && et < BLOCK_N) s_cs[et] = __ldg(p.ln_colsum + n0 + et);
   {
@@ -140,14 +138,21 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     issue_slab(kb_begin);
     for (int kb = kb_begin + 1; kb < kb_end; ++kb) {
       issue_slab(kb);
-      wgmma_wait<1>();  // the previous slab's MMAs have retired: its slot goes back to the producer
+      wgmma_wait<1>();  // the previous slab's MMAs have retired: this warpgroup releases its slot
       fence_regs(acc);
-      if ((et & 127) == 0) mbar_arrive(&empty_bar[(kb - 1 - kb_begin) % STAGES]);
+      // Each use of a slot adds 2 to its counter, one per warpgroup: the leader that finds it odd released last, both
+      // warpgroups have read the slot, and that leader refills it. Nobody waits.
+      if ((et & 127) == 0 && kb - 1 + STAGES < kb_end) {
+        __threadfence_block();
+        const uint32_t before = atomicAdd(&released[(kb - 1 - kb_begin) % STAGES], 1u);
+        __threadfence_block();
+        if (before & 1u) load_slab(kb - 1 + STAGES);
+      }
     }
     wgmma_wait<0>();
     fence_regs(acc);
     // every MMA of both warpgroups has read its operands before the ring is overwritten with the accumulators
-    named_bar_sync(1, GEMM_CONSUMERS);
+    named_bar_sync(1, GEMM_THREADS);
     // fragment of m64nN: thread (warp w, lane l) holds rows 16w + l/4 (+8), columns 8j + 2(l%4) (+1)
     const int r0 = wg * 64 + ((et >> 5) & 3) * 16 + (lane >> 2);
     const int cb = 2 * (lane & 3);
@@ -157,7 +162,7 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       *reinterpret_cast<float2*>(sacc + (r0 + 8) * ACC_LD + 8 * j + cb) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
     }
   }
-  named_bar_sync(1, GEMM_CONSUMERS);
+  named_bar_sync(1, GEMM_THREADS);
 
   // ------------------------------ epilogue -----------------------------------
   const int row = et & 127;
@@ -208,12 +213,22 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       }
     }
   } else if constexpr (EPI_TMA) {
-    if (p.residual) mbar_wait(res_full_bar, 0);
+    // The tile leaves in [128][32] sub-tiles: the two threads of a row fill one 16-column chunk each, thread 0 hands the
+    // sub-tile to a TMA store, and the next sub-tile goes to the other staging buffer while that store reads this one.
+    static_assert(NCH % 2 == 0, "a sub-tile is one chunk of each of a row's two threads");
     const uint32_t sw = uint32_t((row >> 1) & 3);  // SWIZZLE_64B: 16-byte chunk index ^= address bits [7,9)
     float st_s = 0.f, st_q = 0.f;                   // row statistics of this thread's chunks = slot `half`
+    // rows past M are computed and clipped by the TMA store: they read no residual
+    const uint16_t* res_row =
+        p.residual && m < p.M ? static_cast<const uint16_t*>(p.residual) + (long long)m * p.res_ld + n0 : nullptr;
 #pragma unroll 1
     for (int ci = half; ci < NCH; ci += 2) {
       const int c = ci * 16;
+      uint4 r0 = make_uint4(0u, 0u, 0u, 0u), r1 = r0;
+      if (res_row) {
+        r0 = __ldg(reinterpret_cast<const uint4*>(res_row + c));
+        r1 = __ldg(reinterpret_cast<const uint4*>(res_row + c) + 1);
+      }
       float o[16];
       load16(c, o);
       if (p.ln_stats) {
@@ -235,12 +250,13 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
         for (int e = 0; e < 16; ++e) o[e] = gelu_erf_f(o[e]);
       }
-      uint8_t* srow = staging + (c >> 5) * SUB_BYTES + row * 64;
+      const int sub = c >> 5;
+      uint8_t* sbuf = staging + (sub & 1) * GEMM_SUB_BYTES;
+      uint8_t* srow = sbuf + row * 64;
       const uint32_t q0 = uint32_t((c >> 4) & 1) * 2;  // first 16-byte chunk of this 16-column group in the 64 B row
       uint4* s0 = reinterpret_cast<uint4*>(srow + (((q0 + 0) ^ sw) << 4));
       uint4* s1 = reinterpret_cast<uint4*>(srow + (((q0 + 1) ^ sw) << 4));
-      if (p.residual) {
-        const uint4 r0 = *s0, r1 = *s1;
+      if (p.residual) {  // rows past M add the zeros above
         float2 f;
         f = unpack2<BF16>(r0.x); o[0] += f.x; o[1] += f.y;
         f = unpack2<BF16>(r0.y); o[2] += f.x; o[3] += f.y;
@@ -262,17 +278,18 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                        pack2<BF16>(o[6], o[7]));
       *s1 = make_uint4(pack2<BF16>(o[8], o[9]), pack2<BF16>(o[10], o[11]), pack2<BF16>(o[12], o[13]),
                        pack2<BF16>(o[14], o[15]));
+      fence_proxy_async_smem();  // generic-proxy writes -> visible to the TMA store
+      // the previous sub-tile's store has read its buffer before anyone passes this barrier and refills it
+      if (et == 0) tma_store_wait_read();
+      named_bar_sync(1, GEMM_THREADS);
+      if (et == 0) {
+        tma_store_2d(&tmC, sbuf, n0 + sub * 32, m0);
+        tma_store_commit();
+      }
     }
     if (p.row_stats && m < p.M)
       reinterpret_cast<float2*>(p.row_stats)[(long long)m * p.stat_slots + n_tile * 2 + half] = make_float2(st_s, st_q);
-    fence_proxy_async_smem();  // generic-proxy writes -> visible to the TMA store
-    named_bar_sync(1, GEMM_CONSUMERS);
-    if (et == 0) {
-#pragma unroll
-      for (int sub = 0; sub < BLOCK_N / 32; ++sub) tma_store_2d(&tmC, staging + sub * SUB_BYTES, n0 + sub * 32, m0);
-      tma_store_commit();
-      tma_store_wait_read();  // shared memory must outlive the store's reads
-    }
+    if (et == 0) tma_store_wait_read();  // shared memory must outlive the last store's reads
   } else if (p.act == PF_ACT_GEGLU) {
     constexpr int HALF_N = BLOCK_N / 2;
     const int on0 = n_tile * HALF_N;
@@ -460,9 +477,10 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const GemmKernelPara
   }
 }
 
-template <int BLOCK_N, int STAGES, bool EPI_TMA>
+// CTAS: CTAs per SM the instantiation is built for (register cap of the build, shared-memory budget, checked below)
+template <int BLOCK_N, int STAGES, int CTAS, bool EPI_TMA>
 static int launch_gemm(const pf_gemm_args* a, const GemmKernelParams& kp, cudaStream_t st) {
-  CUtensorMap tmA, tmB, tmC, tmR;
+  CUtensorMap tmA, tmB, tmC;
   {
     uint64_t dims[2] = {(uint64_t)a->Kc, (uint64_t)a->a_rows};
     uint64_t str[1] = {(uint64_t)a->a_ld * 2};
@@ -478,33 +496,39 @@ static int launch_gemm(const pf_gemm_args* a, const GemmKernelParams& kp, cudaSt
     if (rc) return rc;
   }
   tmC = tmA;
-  tmR = tmA;
   if constexpr (EPI_TMA) {
     uint64_t dims[2] = {(uint64_t)a->N, (uint64_t)a->M};
     uint32_t box[2] = {32, GEMM_BLOCK_M};
     uint64_t str[1] = {(uint64_t)a->out_ld * 2};
     int rc = make_tmap(&tmC, a->dtype, 2, a->out, dims, str, box, 64);
     if (rc) return rc;
-    if (a->residual) {
-      uint64_t rstr[1] = {(uint64_t)a->res_ld * 2};
-      rc = make_tmap(&tmR, a->dtype, 2, a->residual, dims, rstr, box, 64);
-      if (rc) return rc;
-    }
   }
   constexpr int SMEM = gemm_smem_bytes(BLOCK_N, STAGES, EPI_TMA);
   static_assert(SMEM <= 227 * 1024, "shared memory budget of one H100 CTA");
+  static_assert(CTAS == 1 || SMEM <= GEMM_SMEM_CORESIDENT, "two CTAs per SM: 113 KB of shared memory each");
   const int m_tiles = (a->M + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M;
   const dim3 grid(m_tiles * (a->N / BLOCK_N), kp.k_splits > 1 ? kp.k_splits : 1);
   const int bf = a->dtype == PF_BF16;
-  auto kern = bf ? gemm_taps_kernel<BLOCK_N, STAGES, true, EPI_TMA> : gemm_taps_kernel<BLOCK_N, STAGES, false, EPI_TMA>;
+  auto kern = bf ? gemm_taps_kernel<BLOCK_N, STAGES, CTAS, true, EPI_TMA>
+                 : gemm_taps_kernel<BLOCK_N, STAGES, CTAS, false, EPI_TMA>;
   static bool attr_set[2] = {false, false};  // per dtype: the two kernels share this function's statics
   if (!attr_set[bf]) {
     int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM),
                         "cudaFuncSetAttribute(gemm)");
     if (rc) return rc;
+    // the registers and shared memory this build came out with must admit the CTAs per SM the schedule relies on
+    int resident = 0;
+    rc = check_cuda(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kern, GEMM_THREADS, SMEM),
+                    "cudaOccupancyMaxActiveBlocksPerMultiprocessor(gemm)");
+    if (rc) return rc;
+    if (resident < CTAS) {
+      set_error("gemm_taps_kernel<%d, %d, %s>: %d CTA(s) per SM fit, built for %d", BLOCK_N, STAGES,
+                EPI_TMA ? "tma" : "direct", resident, CTAS);
+      return PF_ERR_UNSUPPORTED;
+    }
     attr_set[bf] = true;
   }
-  kern<<<grid, GEMM_THREADS, SMEM, st>>>(tmA, tmB, tmC, tmR, kp);
+  kern<<<grid, GEMM_THREADS, SMEM, st>>>(tmA, tmB, tmC, kp);
   PF_CHECK_LAUNCH("gemm_taps_kernel");
   return PF_OK;
 }
@@ -656,10 +680,11 @@ extern "C" int pf_gemm_taps(const pf_gemm_args* a, void* stream) {
   if (kp.k_splits > 1) {
     int rc;
     switch (bn) {
-      case 64: rc = launch_gemm<64, 8, false>(a, kp, st); break;
-      case 128: rc = launch_gemm<128, 6, false>(a, kp, st); break;
-      case 160: rc = launch_gemm<160, 5, false>(a, kp, st); break;
-      default: rc = launch_gemm<256, 4, false>(a, kp, st); break;
+      // few tiles of 90-360 K-slabs, planned at about one CTA per SM: nothing to co-schedule, so the long rings
+      case 64: rc = launch_gemm<64, 8, 1, false>(a, kp, st); break;
+      case 128: rc = launch_gemm<128, 6, 1, false>(a, kp, st); break;
+      case 160: rc = launch_gemm<160, 5, 1, false>(a, kp, st); break;
+      default: rc = launch_gemm<256, 4, 1, false>(a, kp, st); break;
     }
     if (rc) return rc;
     const long long total = (long long)a->M * (a->N / 8);
@@ -673,16 +698,16 @@ extern "C" int pf_gemm_taps(const pf_gemm_args* a, void* stream) {
                        (!a->residual || a->res_dtype == a->dtype) && bn != 256;
   if (epi_tma) {
     switch (bn) {
-      case 64: return launch_gemm<64, 8, true>(a, kp, st);
-      case 128: return launch_gemm<128, 5, true>(a, kp, st);
-      case 160: return launch_gemm<160, 5, true>(a, kp, st);
+      case 64: return launch_gemm<64, 4, 2, true>(a, kp, st);
+      case 128: return launch_gemm<128, 3, 2, true>(a, kp, st);
+      case 160: return launch_gemm<160, 3, 2, true>(a, kp, st);
     }
   }
   switch (bn) {
-    case 64: return launch_gemm<64, 8, false>(a, kp, st);
-    case 128: return launch_gemm<128, 6, false>(a, kp, st);
-    case 160: return launch_gemm<160, 5, false>(a, kp, st);
-    case 256: return launch_gemm<256, 4, false>(a, kp, st);
+    case 64: return launch_gemm<64, 4, 2, false>(a, kp, st);
+    case 128: return launch_gemm<128, 3, 2, false>(a, kp, st);
+    case 160: return launch_gemm<160, 3, 2, false>(a, kp, st);
+    case 256: return launch_gemm<256, 4, 1, false>(a, kp, st);
   }
   return PF_ERR_UNSUPPORTED;
 }
