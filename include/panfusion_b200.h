@@ -107,12 +107,13 @@ int pf_p2e(const void* src, void* dst, uint8_t* mask, int dtype, int B, int C, i
  *   map_mode 1: m -> (img, i, j) with i = (m / Wm) % Hm, j = m % Wm; valid iff i0 <= i < i0+Hout and
  *               j0 <= j < j0+Wout; row(m) = (img*Hout + i-i0)*Wout + (j-j0); group(m) = img
  * act: PF_ACT_GEGLU expects B (and bias) packed so that every block_n-wide column tile holds block_n/2 value
- * columns followed by their block_n/2 gate columns; it writes N/2 output columns.
+ * columns followed by their block_n/2 gate columns; it writes N/2 output columns. PF_ACT_GELU is erf-GELU (F.gelu),
+ * PF_ACT_QUICK_GELU is CLIP's x * sigmoid(1.702 x); both apply wherever PF_ACT_SILU does (epilogues, split-K reduce).
  * Constraints: Kc % 64 == 0, N % block_n == 0, block_n in {64,128,160,256}, a_ld/b_ld % 8 == 0.
  * Alignment (checked, PF_ERR_INVALID otherwise): A, B, out, residual, rowbias, splitk_ws and ln_stats 16 bytes;
  * row_stats_out 8 bytes; out_ld, res_ld % 8 == 0 and rowbias_ld % 4 == 0 (elements), so every row stays aligned.
  * ------------------------------------------------------------------------------------------------ */
-enum { PF_ACT_NONE = 0, PF_ACT_SILU = 1, PF_ACT_GELU = 2, PF_ACT_GEGLU = 3 };
+enum { PF_ACT_NONE = 0, PF_ACT_SILU = 1, PF_ACT_GELU = 2, PF_ACT_GEGLU = 3, PF_ACT_QUICK_GELU = 4 };
 #define PF_MAX_TAPS 16
 
 typedef struct pf_gemm_args {
@@ -453,6 +454,34 @@ int pf_inception_head(const float* x, int B, int HW, int C, const float* fc_w, i
 long long pf_inception_score_ws_doubles(int n, int C, int splits);
 int pf_inception_score(const float* logits, const long long* perm, int n, int C, int splits, double* ws, float* out,
                        void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * CLIP score (models/pano/EvalPanoGen.py:33-46: torchmetrics CLIPScore('openai/clip-vit-base-patch16') over
+ * transformers' CLIPProcessor / CLIPModel). Both towers' layers run on pf_gemm_taps (PF_ACT_QUICK_GELU) and pf_fmha_fwd.
+ * pf_clip_prep_taps (host only, no CUDA call): the tap table of CLIPImageProcessor's resize for an H x W image — short
+ *   side to 224, long side to int(224 * long / short) (no resample when the short side is 224) with Pillow's 8-bit
+ *   bicubic filter — restricted to the 224 columns and rows the centre crop keeps (left = (Wr - 224) / 2, top =
+ *   (Hr - 224) / 2). taps: host, pf_clip_prep_taps_ints(H, W) ints = {Kx, Ky, 0, 0}, then per kept column (start,
+ *   count, Kx coefficients), then per kept row (start, count, Ky coefficients); coefficients in 22-bit fixed point.
+ * pf_clip_prep: src [B, 3, H, W] uint8 (is_u8 = 1) or fp32 in [0, 1] (is_u8 = 0: converted per pixel as
+ *   uint8(x * 255), truncated) and taps (device copy of pf_clip_prep_taps(H, W)) -> out [B * 196, 768], fp16 or fp32
+ *   (out_dtype): row b * 196 + py * 14 + px is patch (py, px) of the normalised 224 x 224 crop in the (c, kh, kw) order
+ *   of patch_embedding.weight.reshape(768, -1). The resample is integer-only (bit-identical to PIL.Image.resize), the
+ *   intermediate image never leaves registers; then x / 255 in fp64 rounded to fp32 and (x - mean) / std in fp32.
+ * pf_clip_embed: patches fp32 [B * 196, C] (the patch-embedding GEMM) -> out 16-bit [B * 197, C] =
+ *   pre_layrnorm(cat(class_emb, patches) + pos_emb) per image (class_emb [C], pos_emb [197, C], gamma, beta fp32), and
+ *   row_stats [B * 197][2][2] = (sum, sum of squares, 0, 0) of each stored row, the ln_stats of layer 0's folded LN1
+ *   (the layout of pf_embed_tokens). C % 64 == 0, C <= 1024.
+ * pf_clip_score: img_emb, txt_emb fp32 [B, D] -> scores fp32 [B] = 100 * <img / |img|, txt / |txt|> in fp32, and
+ *   score_sum[0] (fp64, device) += the scores summed in sample order: repeated runs give identical bits. */
+int pf_clip_prep_taps_ints(int H, int W);
+int pf_clip_prep_taps(int H, int W, int* taps);
+int pf_clip_prep(const void* src, int is_u8, int B, int H, int W, const int* taps, void* out, int out_dtype,
+                 void* stream);
+int pf_clip_embed(const float* patches, const float* class_emb, const float* pos_emb, const float* gamma,
+                  const float* beta, float eps, int B, int C, void* out, int dtype, float* row_stats, void* stream);
+int pf_clip_score(const float* img_emb, const float* txt_emb, int B, int D, float* scores, double* score_sum,
+                  void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * View-sharded step (SURVEY.md 8e): device-initiated all-gather over NVLink peer mappings, capturable in a CUDA graph.

@@ -12,7 +12,7 @@ import os
 import torch
 
 PF_F32, PF_F16, PF_BF16 = 0, 1, 2
-PF_ACT_NONE, PF_ACT_SILU, PF_ACT_GELU, PF_ACT_GEGLU = 0, 1, 2, 3
+PF_ACT_NONE, PF_ACT_SILU, PF_ACT_GELU, PF_ACT_GEGLU, PF_ACT_QUICK_GELU = 0, 1, 2, 3, 4
 PF_MAX_TAPS = 16
 PF_CAM_DOUBLES = 20
 
@@ -92,6 +92,7 @@ EXPORTS = [
     "pf_faed_prep", "pf_conv_circ", "pf_faed_pool", "pf_faed_stats", "pf_frechet_ws_doubles", "pf_frechet_fp64",
     "pf_inception_prep", "pf_conv2d_packed_cout", "pf_conv2d_nhwc", "pf_pool2d_nhwc", "pf_inception_head",
     "pf_inception_score_ws_doubles", "pf_inception_score",
+    "pf_clip_prep_taps_ints", "pf_clip_prep_taps", "pf_clip_prep", "pf_clip_embed", "pf_clip_score",
 ]
 
 

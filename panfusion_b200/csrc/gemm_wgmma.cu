@@ -249,6 +249,9 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       } else if (p.act == PF_ACT_GELU) {
 #pragma unroll
         for (int e = 0; e < 16; ++e) o[e] = gelu_erf_f(o[e]);
+      } else if (p.act == PF_ACT_QUICK_GELU) {
+#pragma unroll
+        for (int e = 0; e < 16; ++e) o[e] = quick_gelu_f(o[e]);
       }
       const int sub = c >> 5;
       uint8_t* sbuf = staging + (sub & 1) * GEMM_SUB_BYTES;
@@ -360,6 +363,9 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       } else if (p.act == PF_ACT_GELU) {
 #pragma unroll
         for (int e = 0; e < 16; ++e) o[e] = gelu_erf_f(o[e]);
+      } else if (p.act == PF_ACT_QUICK_GELU) {
+#pragma unroll
+        for (int e = 0; e < 16; ++e) o[e] = quick_gelu_f(o[e]);
       }
       if (p.residual) {
         if (p.res_f32) {
@@ -451,6 +457,9 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const GemmKernelPara
   } else if (p.act == PF_ACT_GELU) {
 #pragma unroll
     for (int e = 0; e < 8; ++e) o[e] = gelu_erf_f(o[e]);
+  } else if (p.act == PF_ACT_QUICK_GELU) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) o[e] = quick_gelu_f(o[e]);
   }
   if (p.residual) {
     if (p.res_f32) {
@@ -605,7 +614,7 @@ extern "C" int pf_gemm_taps(const pf_gemm_args* a, void* stream) {
   PF_CHECK_ARG(a->out_dtype == PF_F32 || a->out_dtype == a->dtype, "pf_gemm_taps: out_dtype must be f32 or dtype");
   PF_CHECK_ARG(!a->residual || a->res_dtype == PF_F32 || a->res_dtype == a->dtype,
                "pf_gemm_taps: res_dtype must be f32 or dtype");
-  PF_CHECK_ARG(a->act >= PF_ACT_NONE && a->act <= PF_ACT_GEGLU, "pf_gemm_taps: unknown act %d", a->act);
+  PF_CHECK_ARG(a->act >= PF_ACT_NONE && a->act <= PF_ACT_QUICK_GELU, "pf_gemm_taps: unknown act %d", a->act);
   // block_n: low 16 bits = tile width (0 = auto); the high bits are ignored (one schedule)
   int bn = pf::resolve_block_n(a);
   PF_CHECK_ARG(bn == 64 || bn == 128 || bn == 160 || bn == 256, "pf_gemm_taps: unsupported block_n %d (N=%d)", bn, a->N);

@@ -212,6 +212,10 @@ __device__ __forceinline__ float rcp_approx(float x) {
 __device__ __forceinline__ float silu_f(float x) {
   return x * rcp_approx(1.0f + ex2_approx(-1.4426950408889634f * x));
 }
+// CLIP's quick_gelu, x * sigmoid(1.702 x): the same five instructions with the factor 1.702 * log2(e) folded in
+__device__ __forceinline__ float quick_gelu_f(float x) {
+  return x * rcp_approx(1.0f + ex2_approx(-2.4554669595930157f * x));
+}
 // exact-erf GELU (F.gelu default) with erf from Abramowitz & Stegun 7.1.26 (|error| <= 1.5e-7 + MUFU round-off,
 // three orders of magnitude below one 16-bit output ulp): 2 MUFU + 7 FFMA + 5 FMUL + 1 LOP3 instead of erff()'s
 // branchy ~30-instruction sequence — the GEGLU epilogue evaluates it 80x per thread per tile.

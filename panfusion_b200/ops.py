@@ -8,7 +8,8 @@ import torch
 from torch import Tensor
 
 from . import _lib
-from ._lib import PF_ACT_GEGLU, PF_ACT_GELU, PF_ACT_NONE, PF_ACT_SILU, FmhaArgs, GemmArgs  # noqa: F401
+from ._lib import (PF_ACT_GEGLU, PF_ACT_GELU, PF_ACT_NONE, PF_ACT_QUICK_GELU, PF_ACT_SILU, FmhaArgs,  # noqa: F401
+                   GemmArgs)
 
 
 # number of CUDA kernels launched through this module (bench.py reports it as `gpu_launches`)

@@ -39,6 +39,31 @@ class _Layer:
         self.fc2 = _Lin(layer.mlp.fc2.weight, layer.mlp.fc2.bias, dev, dt)
 
 
+# transformers' ACT2FN names of the CLIP MLP -> the tap-GEMM epilogue that applies them
+ACTIVATIONS = {"gelu": ops.PF_ACT_GELU, "quick_gelu": ops.PF_ACT_QUICK_GELU}
+
+
+def encoder_layers(x: Tensor, st: Tensor, layers, B: int, L: int, heads: int, act: int,
+                   bias: Optional[Tensor] = None) -> Tensor:
+    """The pre-LN CLIP encoder layers (CLIPEncoderLayer [3P]) of both towers over x [B*L, C] (16-bit residual stream) with
+    st = its row statistics [B*L, 2, 2]; bias = the attention's additive fp32 bias [L, >=L] (the text tower's causal
+    mask) or None (the vision tower). Returns the residual stream after the last layer."""
+    T, C = x.shape
+    dt, dev = x.dtype, x.device
+    new = lambda n: torch.empty((T, n), dtype=dt, device=dev)
+    for l in layers:
+        qkv = ops.gemm_taps(x, l.qkv.w, new(3 * C), M=T, Kc=C, bias=l.qkv.b,
+                            ln=(st, l.qkv.colsum, l.qkv.eps)).reshape(B, L, 3 * C)
+        o = torch.empty((B, L, C), dtype=dt, device=dev)
+        ops.fmha(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], o, heads=heads, head_dim=64, scale=64 ** -0.5,
+                 bias=bias)
+        x, st = ops.gemm_taps(o.reshape(T, C), l.out.w, new(C), M=T, Kc=C, bias=l.out.b, residual=x, row_stats=True)
+        h = ops.gemm_taps(x, l.fc1.w, new(l.fc1.n), M=T, Kc=C, bias=l.fc1.b, act=act,
+                          ln=(st, l.fc1.colsum, l.fc1.eps))
+        x, st = ops.gemm_taps(h, l.fc2.w, new(C), M=T, Kc=l.fc2.k, bias=l.fc2.b, residual=x, row_stats=True)
+    return x
+
+
 class CLIPTextEncoder:
     """`text_encoder(input_ids)[0]` of a duck-typed transformers `CLIPTextModel` (anything exposing
     `.text_model.{embeddings.{token_embedding,position_embedding}, encoder.layers[i].{layer_norm1, self_attn.{q,k,v,out}_proj,
@@ -58,8 +83,9 @@ class CLIPTextEncoder:
         tm = self.src.text_model
         cfg = self.src.config
         act = getattr(cfg, "hidden_act", "gelu")
-        if act != "gelu":
-            raise NotImplementedError(f"CLIP text encoder with hidden_act={act!r}: SD-2's tower uses erf-GELU (PF_ACT_GELU)")
+        if act not in ACTIVATIONS:
+            raise NotImplementedError(f"CLIP text encoder with hidden_act={act!r}: 'gelu' (SD-2's tower, PF_ACT_GELU) "
+                                      "and 'quick_gelu' (OpenAI CLIP, PF_ACT_QUICK_GELU) are served")
         heads = int(cfg.num_attention_heads)
         C = int(cfg.hidden_size)
         if C // heads != 64:
@@ -72,7 +98,7 @@ class CLIPTextEncoder:
         bias = torch.zeros((L, ld), dtype=torch.float32)
         bias[:, :L] = torch.full((L, L), torch.finfo(torch.float32).min).triu(1)
         self._packed = dict(
-            dev=dev, dt=dt, C=C, heads=heads, L=L, vocab=tm.embeddings.token_embedding.weight.shape[0],
+            dev=dev, dt=dt, C=C, heads=heads, L=L, act=ACTIVATIONS[act], vocab=tm.embeddings.token_embedding.weight.shape[0],
             tok=f32(tm.embeddings.token_embedding.weight), pos=f32(tm.embeddings.position_embedding.weight),
             layers=[_Layer(l, dev, dt) for l in tm.encoder.layers], final=_Norm(tm.final_layer_norm, dev),
             causal=bias.to(dev))
@@ -90,24 +116,14 @@ class CLIPTextEncoder:
         if Lx > L:
             raise ValueError(f"sequence length {Lx} exceeds max_position_embeddings {L}")
         T = B * Lx
-        new = lambda n: torch.empty((T, n), dtype=dt, device=dev)
-        x = new(C)
+        x = torch.empty((T, C), dtype=dt, device=dev)
         st = torch.empty((T, 2, 2), dtype=torch.float32, device=dev)
         Cv = _lib.C.c_void_p
         ops._count(1)
         _lib.check(_lib.lib().pf_embed_tokens(Cv(ids.data_ptr()), Cv(w["tok"].data_ptr()), Cv(w["pos"].data_ptr()),
                                               Cv(x.data_ptr()), _lib.dtype_code(dt), Cv(st.data_ptr()), T, Lx, C, w["vocab"],
                                               Cv(_lib.stream_ptr())))
-        bias = w["causal"][:Lx]
-        for l in w["layers"]:
-            qkv = ops.gemm_taps(x, l.qkv.w, new(3 * C), M=T, Kc=C, bias=l.qkv.b,
-                                ln=(st, l.qkv.colsum, l.qkv.eps)).reshape(B, Lx, 3 * C)
-            o = torch.empty((B, Lx, C), dtype=dt, device=dev)
-            ops.fmha(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], o, heads=H, head_dim=64, scale=64 ** -0.5, bias=bias)
-            x, st = ops.gemm_taps(o.reshape(T, C), l.out.w, new(C), M=T, Kc=C, bias=l.out.b, residual=x, row_stats=True)
-            h = ops.gemm_taps(x, l.fc1.w, new(l.fc1.n), M=T, Kc=C, bias=l.fc1.b, act=ops.PF_ACT_GELU,
-                              ln=(st, l.fc1.colsum, l.fc1.eps))
-            x, st = ops.gemm_taps(h, l.fc2.w, new(C), M=T, Kc=l.fc2.k, bias=l.fc2.b, residual=x, row_stats=True)
+        x = encoder_layers(x, st, w["layers"], B, Lx, H, w["act"], bias=w["causal"][:Lx])
         out = ops.layernorm(x, w["final"].g, w["final"].b, w["final"].eps)
         return out.reshape(B, Lx, C)
 
