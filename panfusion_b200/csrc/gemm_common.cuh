@@ -6,10 +6,26 @@ namespace pf {
 
 constexpr int GEMM_BLOCK_M = 128;
 constexpr int GEMM_BLOCK_K = 64;  // 64 x 16-bit = 128 B = one swizzle row
+// Taps whose offsets lie within GEMM_WIN_SPAN rows of each other share one A window of 128 + GEMM_WIN_SPAN rows.
+// 8 covers a 3x3 kernel row (span 2) and an Upsample2D phase row (span 1) and keeps two windows and three 160-wide B
+// boxes inside a co-resident CTA's 108 KB ring.
+constexpr int GEMM_WIN_SPAN = 8;
+constexpr int GEMM_WIN_BYTES = (GEMM_BLOCK_M + GEMM_WIN_SPAN) * GEMM_BLOCK_K * 2;
 
 struct GemmKernelParams {
-  int M, N, num_kb, kb_per_tap;
-  int tap_off[PF_MAX_TAPS];
+  int M, N, kb_per_tap;
+  // K order: (window group, 64-channel slab, tap of the group). Taps are sorted by offset; group g holds sorted taps
+  // [grp_first[g], grp_first[g + 1]) and its A window starts grp_off[g] rows from the tile. A unit is one
+  // (group, channel slab) pair: one A window and one B box per tap of the group.
+  int num_groups, num_units;
+  int grp_first[PF_MAX_TAPS + 1];
+  int grp_off[PF_MAX_TAPS];
+  int tap_src[PF_MAX_TAPS];    // sorted tap: the caller's tap index, i.e. its block of B's columns
+  // the operand ring: a_slots A windows of a_rows rows, then the B boxes. slab_ring: every group is a single tap, so
+  // each K-slab's A box travels with its B box (one barrier per slot, as a plain GEMM's ring)
+  int a_rows, a_slots, slab_ring;
+  // group g: the rows its taps start past the window start (0..GEMM_WIN_SPAN), 4 bits per tap in sorted order
+  unsigned long long grp_shifts[PF_MAX_TAPS];
   void* out;
   int out_ld;
   int out_f32;

@@ -3,7 +3,11 @@
 // (reference call sites: models/pano/MVGenModel.py:85-295 through diffusers ResnetBlock2D / Transformer2DModel,
 //  models/modules/transformer.py:57-74,8-35). A convolution is a sum of `num_taps` GEMMs whose A operand is the
 // same channels-last image shifted by a constant row offset (zero-haloed "padded-flat" layout), so the im2col
-// matrix is never formed: each K-slab is one plain 2-D TMA box.
+// matrix is never formed. Taps whose offsets lie within GEMM_WIN_SPAN (8) rows of each other (the three taps of a 3x3
+// kernel row) read one A window of 128 + 8 rows, fetched once per 64-channel slab with one 2-D TMA box, and each tap's
+// wgmma A operand starts 0..8 rows into it; only the B box is fetched per tap. A 3x3 convolution's tile so reads each
+// A row 3 times per channel slab from L2 instead of 9. A GEMM whose taps are all further apart (linears, 1x1
+// convolutions) runs the plain slab ring: one A box and one B box per K-slab behind one barrier.
 //
 // 256 threads: warps 0..3 and 4..7 = two warpgroups, each owning 64 of the 128 tile rows through the main loop.
 // There is no producer warp: thread 0 fills the ring before the loop, and the leader of whichever warpgroup releases
@@ -43,8 +47,9 @@ __host__ __device__ constexpr int gemm_ring_bytes(int block_n, int stages, bool 
   const int epi = gemm_acc_bytes(block_n) + (epi_tma ? 2 * GEMM_SUB_BYTES : 0);
   return ((ring > epi ? ring : epi) + 1023) / 1024 * 1024;
 }
-// full barrier (8 bytes) and release counter (4 bytes) per stage, rounded up to keep s_bias 16-byte aligned
-__host__ __device__ constexpr int gemm_bar_bytes(int stages) { return (stages * 12 + 15) / 16 * 16; }
+// full barrier (8 bytes) and release counter (4 bytes) per A slot and per B slot (at most STAGES of each), rounded up
+// to keep s_bias 16-byte aligned
+__host__ __device__ constexpr int gemm_bar_bytes(int stages) { return (2 * stages * 12 + 15) / 16 * 16; }
 __host__ __device__ constexpr int gemm_smem_bytes(int block_n, int stages, bool epi_tma) {
   return gemm_ring_bytes(block_n, stages, epi_tma) + gemm_bar_bytes(stages) +
          2 * block_n * 4 /*bias row + LayerNorm column sums*/;
@@ -54,8 +59,7 @@ template <int BLOCK_N, int STAGES, int CTAS, bool BF16, bool EPI_TMA>
 __global__ void __launch_bounds__(GEMM_THREADS, CTAS)
 gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmC, const GemmKernelParams p) {
-  constexpr int A_BYTES = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;
-  constexpr int STAGE_BYTES = gemm_stage_bytes(BLOCK_N);
+  constexpr int B_BYTES = BLOCK_N * GEMM_BLOCK_K * 2;
   constexpr int RING_BYTES = gemm_ring_bytes(BLOCK_N, STAGES, EPI_TMA);
   constexpr int ACC_LD = gemm_acc_ld(BLOCK_N);
   constexpr int NCH = BLOCK_N / 16;
@@ -67,10 +71,15 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   float* sacc = reinterpret_cast<float*>(smem);  // [128][ACC_LD] fp32, over the ring once the main loop is done
   uint8_t* staging = smem + gemm_acc_bytes(BLOCK_N);  // EPI_TMA: two [128][32] 16-bit sub-tiles, also inside the ring
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + RING_BYTES);
-  uint32_t* released = reinterpret_cast<uint32_t*>(full_bar + STAGES);  // per slot: releases by the two warpgroups
+  // the ring: p.a_slots A windows, then STAGES B boxes (1024-byte multiples, so every slot is swizzle-aligned)
+  const int a_bytes = p.a_rows * (GEMM_BLOCK_K * 2);
+  uint8_t* const b_ring = smem + p.a_slots * a_bytes;
+  uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + RING_BYTES);
+  uint64_t* b_full = a_full + STAGES;
+  uint32_t* a_rel = reinterpret_cast<uint32_t*>(b_full + STAGES);  // per slot: releases by the two warpgroups
+  uint32_t* b_rel = a_rel + STAGES;
   float* s_bias = reinterpret_cast<float*>(smem + RING_BYTES + gemm_bar_bytes(STAGES));  // [BLOCK_N]
-  float* s_cs = s_bias + BLOCK_N;                                            // [BLOCK_N] LayerNorm column sums
+  float* s_cs = s_bias + BLOCK_N;  // [BLOCK_N] LayerNorm column sums
 
   const int et = threadIdx.x;  // 0..255
   const int lane = et & 31;
@@ -79,36 +88,75 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int n_tile = int(blockIdx.x) % n_tiles;  // n fastest: concurrent CTAs share the A tile through L2
   const int m0 = (int(blockIdx.x) / n_tiles) * GEMM_BLOCK_M;
   const int n0 = n_tile * BLOCK_N;
-  // split-K: this CTA owns K-slabs [kb_begin, kb_end)
+  const int kpt = p.kb_per_tap;
+  // split-K: this CTA owns units [u_begin, u_end), i.e. K-slabs [s_begin, s_end)
   const int split = p.k_splits > 1 ? int(blockIdx.y) : 0;
-  const int kb_begin = (p.k_splits > 1) ? (int)((long long)split * p.num_kb / p.k_splits) : 0;
-  const int kb_end = (p.k_splits > 1) ? (int)((long long)(split + 1) * p.num_kb / p.k_splits) : p.num_kb;
+  const int u_begin = (p.k_splits > 1) ? (int)((long long)split * p.num_units / p.k_splits) : 0;
+  const int u_end = (p.k_splits > 1) ? (int)((long long)(split + 1) * p.num_units / p.k_splits) : p.num_units;
+  auto first_slab = [&](int u) {  // K-slab of unit u's first tap (u = num_units: the end of K)
+    const int gu = u / kpt, ku = u - gu * kpt;
+    return p.grp_first[gu] * kpt + (ku ? ku * (p.grp_first[gu + 1] - p.grp_first[gu]) : 0);
+  };
+  const int s_begin = first_slab(u_begin), s_end = first_slab(u_end);
 
   if (et == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      released[s] = 0u;
+      mbar_init(&a_full[s], 1);
+      mbar_init(&b_full[s], 1);
+      a_rel[s] = b_rel[s] = 0u;
     }
     if constexpr (EPI_TMA) tma_prefetch_desc(&tmC);
     fence_barrier_init();
   }
   __syncthreads();
 
-  // one K-slab into its ring slot (one thread): the A box of the slab's tap and the B box of the slab
-  auto load_slab = [&](int kb) {
-    const int s = (kb - kb_begin) % STAGES;
-    const int tap = kb / p.kb_per_tap;
-    const int kk = kb - tap * p.kb_per_tap;
-    uint8_t* sa = smem + s * STAGE_BYTES;
-    mbar_expect_tx(&full_bar[s], STAGE_BYTES);
-    tma_load_2d(sa, &tmA, &full_bar[s], kk * GEMM_BLOCK_K, m0 + p.tap_off[tap]);
-    tma_load_2d(sa + A_BYTES, &tmB, &full_bar[s], kb * GEMM_BLOCK_K, n0);
+  // Where K-slab s sits in the K order: sorted tap i of group g at channel slab kk. The main loop never calls this: it
+  // walks the order incrementally, so no division or table search lies between two slabs' MMAs.
+  auto locate = [&](int s, int& gs, int& ks, int& is) {
+    gs = 0;
+    while (s >= p.grp_first[gs + 1] * kpt) ++gs;
+    const int taps = p.grp_first[gs + 1] - p.grp_first[gs];
+    const int r = s - p.grp_first[gs] * kpt;
+    ks = r / taps;
+    is = p.grp_first[gs] + r - ks * taps;
+  };
+  // One thread each: the A window of group ga at channel slab ka, and the B box of sorted tap ib at channel slab kb
+  // (group gb). In a slab ring (every group a single tap, so units are slabs) a slab's A box and B box share slot and
+  // barrier, and the A barriers and counters stay unused.
+  auto load_a = [&](int slot, int ga, int ka, uint64_t* bar) {
+    tma_load_2d(smem + slot * a_bytes, &tmA, bar, ka * GEMM_BLOCK_K, m0 + p.grp_off[ga]);
+  };
+  auto fill_a = [&](int slot, int ga, int ka) {
+    mbar_expect_tx(&a_full[slot], a_bytes);
+    load_a(slot, ga, ka, &a_full[slot]);
+  };
+  auto fill_b = [&](int slot, int gb, int kb, int ib) {
+    mbar_expect_tx(&b_full[slot], B_BYTES + (p.slab_ring ? a_bytes : 0));
+    if (p.slab_ring) load_a(slot, gb, kb, &b_full[slot]);
+    tma_load_2d(b_ring + slot * B_BYTES, &tmB, &b_full[slot], (p.tap_src[ib] * kpt + kb) * GEMM_BLOCK_K, n0);
   };
   if (et == 0) {
-    for (int kb = kb_begin; kb < kb_end && kb < kb_begin + STAGES; ++kb) load_slab(kb);
+    if (!p.slab_ring)
+      for (int k = 0; k < p.a_slots && u_begin + k < u_end; ++k) {
+        const int gu = (u_begin + k) / kpt;
+        fill_a(k, gu, u_begin + k - gu * kpt);
+      }
+    for (int k = 0; k < STAGES && s_begin + k < s_end; ++k) {
+      int gs, ks, is;
+      locate(s_begin + k, gs, ks, is);
+      fill_b(k, gs, ks, is);
+    }
   }
+  // Each use of a slot adds 2 to its counter, one per warpgroup: the leader that finds it odd released last, both
+  // warpgroups have read the slot, and that leader refills it. Nobody waits.
+  auto released_last = [](uint32_t* counter) {
+    __threadfence_block();
+    const uint32_t before = atomicAdd(counter, 1u);
+    __threadfence_block();
+    return (before & 1u) != 0u;
+  };
 
   // ------------------------------ main loop ------------------------------
   if (p.bias && et < BLOCK_N) s_bias[et] = __ldg(p.bias + n0 + et);
@@ -117,13 +165,30 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     float acc[NACC];
 #pragma unroll
     for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+    // The MMA walk: K-slab s is tap t of group g (gsize taps, row shifts packed 4 bits per tap in gshift) at channel
+    // slab kk; its A window and B box sit in ring slots a_slot / b_slot, whose barriers complete with parity a_par /
+    // b_par. Every thread keeps the same walks, so whichever leader releases a slot last can refill it.
+    int g = u_begin / kpt, kk = u_begin - g * kpt, t = 0;
+    int gsize = p.grp_first[g + 1] - p.grp_first[g];
+    uint64_t gshift = p.grp_shifts[g];
+    int a_slot = 0, a_par = 0, b_slot = 0, b_par = 0;
+    // The B load walk: the next B box to load, K-slab s + STAGES - 1 at step s, is sorted tap ib (of [ib0, ib_end),
+    // group gb) at channel slab kb.
+    int gb = 0, kb = 0, ib = 0;
+    if (s_begin + STAGES < s_end) locate(s_begin + STAGES, gb, kb, ib);
+    int ib0 = p.grp_first[gb], ib_end = p.grp_first[gb + 1];
+    // The window load walk: the next window to load is unit ua, group ga at channel slab ka.
+    int ua = u_begin + p.a_slots, ga = ua / kpt, ka = ua - ga * kpt;
     // issue one K-slab's MMAs as one commit group (every range holds at least one slab)
-    auto issue_slab = [&](int kb) {
-      const int s = (kb - kb_begin) % STAGES;
-      mbar_wait(&full_bar[s], ((kb - kb_begin) / STAGES) & 1);
-      const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
-      const uint64_t adesc = make_wgmma_desc(sa + wg * (64 * 128), 16, 1024, 1);
-      const uint64_t bdesc = make_wgmma_desc(sa + A_BYTES, 16, 1024, 1);
+    auto issue_slab = [&]() {
+      if (!p.slab_ring && t == 0) mbar_wait(&a_full[a_slot], a_par);  // the window's first tap
+      mbar_wait(&b_full[b_slot], b_par);
+      // the tap's 128 rows start its shift into the window; the 128 B swizzle follows the shared-memory address, as
+      // the TMA wrote it, so a start that is not 1024-byte aligned needs no base offset
+      const int shift = int(gshift >> (4 * t)) & 15;
+      const uint32_t sa = smem_u32(smem + a_slot * a_bytes) + (shift + wg * 64) * (GEMM_BLOCK_K * 2);
+      const uint64_t adesc = make_wgmma_desc(sa, 16, 1024, 1);
+      const uint64_t bdesc = make_wgmma_desc(smem_u32(b_ring + b_slot * B_BYTES), 16, 1024, 1);
       wgmma_fence();
       fence_regs(acc);
 #pragma unroll
@@ -135,18 +200,52 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     // The first slab is issued before the loop, so the zeroing above never meets an in-flight MMA at the loop head.
     // Without the peel ptxas sees the accumulators defined both by those moves and by MMAs still in flight, and
     // serialises every wgmma (a full wait after each m64 x BLOCK_N x k16, warning C7515).
-    issue_slab(kb_begin);
-    for (int kb = kb_begin + 1; kb < kb_end; ++kb) {
-      issue_slab(kb);
-      wgmma_wait<1>();  // the previous slab's MMAs have retired: this warpgroup releases its slot
+    issue_slab();
+    for (int s = s_begin + 1; s < s_end; ++s) {
+      if (++b_slot == STAGES) {
+        b_slot = 0;
+        b_par ^= 1;
+      }
+      const bool new_window = ++t == gsize;
+      if (new_window) {
+        t = 0;
+        if (++kk == kpt) {
+          kk = 0;
+          ++g;
+          gsize = p.grp_first[g + 1] - p.grp_first[g];
+          gshift = p.grp_shifts[g];
+        }
+        if (++a_slot == p.a_slots) {
+          a_slot = 0;
+          a_par ^= 1;
+        }
+      }
+      issue_slab();
+      wgmma_wait<1>();  // slab s - 1 has retired: this warpgroup releases its B box, and its window if that was its last tap
       fence_regs(acc);
-      // Each use of a slot adds 2 to its counter, one per warpgroup: the leader that finds it odd released last, both
-      // warpgroups have read the slot, and that leader refills it. Nobody waits.
-      if ((et & 127) == 0 && kb - 1 + STAGES < kb_end) {
-        __threadfence_block();
-        const uint32_t before = atomicAdd(&released[(kb - 1 - kb_begin) % STAGES], 1u);
-        __threadfence_block();
-        if (before & 1u) load_slab(kb - 1 + STAGES);
+      const bool load_b = s - 1 + STAGES < s_end;
+      const bool load_a = !p.slab_ring && new_window && ua < u_end;
+      if ((et & 127) == 0) {
+        const int bs = (b_slot ? b_slot : STAGES) - 1;
+        if (load_b && released_last(&b_rel[bs])) fill_b(bs, gb, kb, ib);
+        const int as = (a_slot ? a_slot : p.a_slots) - 1;
+        if (load_a && released_last(&a_rel[as])) fill_a(as, ga, ka);
+      }
+      if (load_b && ++ib == ib_end) {
+        if (++kb == kpt) {
+          kb = 0;
+          ++gb;
+          ib0 = ib_end;
+          ib_end = gb < p.num_groups ? p.grp_first[gb + 1] : ib_end;
+        }
+        ib = ib0;
+      }
+      if (load_a) {
+        ++ua;
+        if (++ka == kpt) {
+          ka = 0;
+          ++ga;
+        }
       }
     }
     wgmma_wait<0>();
@@ -488,12 +587,19 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const GemmKernelPara
 
 // CTAS: CTAs per SM the instantiation is built for (register cap of the build, shared-memory budget, checked below)
 template <int BLOCK_N, int STAGES, int CTAS, bool EPI_TMA>
-static int launch_gemm(const pf_gemm_args* a, const GemmKernelParams& kp, cudaStream_t st) {
+static int launch_gemm(const pf_gemm_args* a, GemmKernelParams kp, cudaStream_t st) {
+  // STAGES B boxes, and as many A windows as the rest of the ring holds (a slab ring: STAGES 128-row boxes)
+  const int a_slots = (gemm_ring_bytes(BLOCK_N, STAGES, EPI_TMA) - STAGES * BLOCK_N * GEMM_BLOCK_K * 2) /
+                      (kp.a_rows * GEMM_BLOCK_K * 2);
+  kp.a_slots = a_slots < STAGES ? a_slots : STAGES;
+  // a window is refilled when the last tap of the window before it has retired: the ring needs two of them
+  static_assert(gemm_ring_bytes(BLOCK_N, STAGES, EPI_TMA) - STAGES * BLOCK_N * GEMM_BLOCK_K * 2 >= 2 * GEMM_WIN_BYTES,
+                "two A windows next to the B boxes");
   CUtensorMap tmA, tmB, tmC;
   {
     uint64_t dims[2] = {(uint64_t)a->Kc, (uint64_t)a->a_rows};
     uint64_t str[1] = {(uint64_t)a->a_ld * 2};
-    uint32_t box[2] = {GEMM_BLOCK_K, GEMM_BLOCK_M};
+    uint32_t box[2] = {GEMM_BLOCK_K, (uint32_t)kp.a_rows};
     int rc = make_tmap(&tmA, a->dtype, 2, a->A, dims, str, box, 128);
     if (rc) return rc;
   }
@@ -640,8 +746,33 @@ extern "C" int pf_gemm_taps(const pf_gemm_args* a, void* stream) {
   kp.M = a->M;
   kp.N = a->N;
   kp.kb_per_tap = a->Kc / GEMM_BLOCK_K;
-  kp.num_kb = kp.kb_per_tap * a->num_taps;
-  for (int t = 0; t < PF_MAX_TAPS; ++t) kp.tap_off[t] = t < a->num_taps ? a->tap_off[t] : 0;
+  // Taps sorted by offset (equal offsets keep the caller's order) and cut into window groups: a tap joins the current
+  // group while it lies within GEMM_WIN_SPAN rows of the group's first. The K order, and so the summation order,
+  // depends on the tap offsets alone, never on M; a one-tap GEMM keeps the plain slab order.
+  int order[PF_MAX_TAPS];
+  for (int t = 0; t < a->num_taps; ++t) {
+    int k = t;
+    for (; k > 0 && a->tap_off[order[k - 1]] > a->tap_off[t]; --k) order[k] = order[k - 1];
+    order[k] = t;
+  }
+  kp.num_groups = 0;
+  for (int k = 0; k < PF_MAX_TAPS; ++k) kp.grp_shifts[k] = 0;
+  int span = 0;
+  for (int k = 0; k < a->num_taps; ++k) {
+    const int off = a->tap_off[order[k]];
+    if (k == 0 || (long long)off - kp.grp_off[kp.num_groups - 1] > GEMM_WIN_SPAN) {
+      kp.grp_first[kp.num_groups] = k;
+      kp.grp_off[kp.num_groups++] = off;
+    }
+    const int shift = off - kp.grp_off[kp.num_groups - 1];
+    kp.grp_shifts[kp.num_groups - 1] |= uint64_t(shift) << (4 * (k - kp.grp_first[kp.num_groups - 1]));
+    kp.tap_src[k] = order[k];
+    span = span > shift ? span : shift;
+  }
+  kp.grp_first[kp.num_groups] = a->num_taps;
+  kp.num_units = kp.num_groups * kp.kb_per_tap;
+  kp.a_rows = GEMM_BLOCK_M + (span ? GEMM_WIN_SPAN : 0);
+  kp.slab_ring = kp.num_groups == a->num_taps;
   kp.out = a->out;
   kp.out_ld = a->out_ld;
   kp.out_f32 = a->out_dtype == PF_F32;
@@ -673,8 +804,8 @@ extern "C" int pf_gemm_taps(const pf_gemm_args* a, void* stream) {
   kp.ln_colsum = a->ln_colsum;
   kp.ln_inv_k = 1.0f / float((long long)a->Kc * a->num_taps);
   kp.ln_eps = a->ln_eps;
-  PF_CHECK_ARG(kp.k_splits == 1 || (a->splitk_ws && a->act != PF_ACT_GEGLU && kp.k_splits <= kp.num_kb),
-               "pf_gemm_taps: split-K needs a workspace, no GEGLU and k_splits <= K-slabs");
+  PF_CHECK_ARG(kp.k_splits == 1 || (a->splitk_ws && a->act != PF_ACT_GEGLU && kp.k_splits <= kp.num_units),
+               "pf_gemm_taps: split-K needs a workspace, no GEGLU and k_splits <= (tap window, channel slab) units");
   const bool fused_ln = a->row_stats_out || a->ln_stats;
   if (fused_ln) {
     PF_CHECK_ARG(kp.k_splits == 1, "pf_gemm_taps: fused LayerNorm does not combine with split-K");

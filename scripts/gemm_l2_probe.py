@@ -4,11 +4,13 @@
 
 Shape: M = 65 536 rows, K = 2 880 as 9 taps x 320 channels (a 3x3 convolution's offsets over a 66-pixel row pitch),
 N = 1 280, bf16, direct-store epilogue at every width (so only the tile width changes). Each CTA computes one
-128 x block_n tile and, per 64-deep K-slab, fills its shared memory with a 16 KB A box and a block_n x 128 B B box.
-The script prints TFLOP/s, FLOP per byte of that fill, and the fill rate (16 KB + block_n * 128 B) * slabs * tiles /
-time. Without multicast every filled byte is read from L2. With the B box multicast to a CTA pair, each pair reads B
-once, so L2 serves (16 KB + block_n * 64 B) per CTA and slab for the same fill. If TFLOP/s rises with FLOP/B while the
-fill rate stays roughly flat, the main loop is L2-bound.
+128 x block_n tile. The taps of one kernel row lie within 2 rows of each other, so they share one A window of
+128 + 8 rows (17 KB) per 64-channel slab, and every tap adds a block_n x 128 B B box: the fill per tile is
+windows * 17 KB + slabs * block_n * 128 B, with 3 windows and 9 slabs per 64 channels. The script prints TFLOP/s,
+FLOP per byte of that fill, and the fill rate (fill per tile * tiles / time). Every filled byte is read from L2. If
+TFLOP/s rises with FLOP/B while the fill rate stays roughly flat, the main loop is L2-bound. For a build that loads a
+16 KB A box per tap (the tap-GEMM before A windows), the "slab" columns give the same accounting for
+(16 KB + block_n * 128 B) per slab.
 
 Timing follows bench.py's micro_rooflines: 20 launches captured in one CUDA graph, rotating over buffer sets larger
 than L2, CUDA events around 25 replays, with the median SM clock sampled by nvidia-smi over the same window.
@@ -59,6 +61,7 @@ def main():
     outs = [torch.empty(M, N, dtype=torch.bfloat16, device=dev) for _ in range(3)]
     flops = 2.0 * M * N * CI * TAPS
     slabs = CI // 64 * TAPS
+    windows = CI // 64 * 3  # one per kernel row and channel slab
     m_tiles = (M + 127) // 128
     rows = []
     for bn in (64, 128, 160, 256):
@@ -66,13 +69,17 @@ def main():
                                                image_map=(1, M, 0, 0, 1, M))) for a, o in zip(As, outs)]
         with ClockSampler(dev.index or 0) as clk:
             ms = timeit(fns, reps=25)
-        fill = (16384 + bn * 128) * slabs * m_tiles * (N // bn)
+        tiles = m_tiles * (N // bn)
+        fill = (windows * (128 + 8) * 128 + slabs * bn * 128) * tiles
+        fill_slab = (16384 + bn * 128) * slabs * tiles
         r = dict(block_n=bn, ms=round(ms, 4), tflops=round(flops / ms / 1e9, 1),
                  flop_per_byte=round(flops / fill, 1), fill_tbs=round(fill / ms / 1e9, 2),
+                 slab_flop_per_byte=round(flops / fill_slab, 1), slab_fill_tbs=round(fill_slab / ms / 1e9, 2),
                  sm_mhz=clk.summary()["sm_mhz"])
         rows.append(r)
-        print(f"block_n={bn:3d}: {ms * 1e3:7.1f} us  {r['tflops']:6.1f} TFLOP/s  {r['flop_per_byte']:5.1f} FLOP/B  "
-              f"{r['fill_tbs']:5.2f} TB/s L2->SMEM fill  (median SM clock {r['sm_mhz']} MHz)")
+        print(f"block_n={bn:3d}: {ms * 1e3:7.1f} us  {r['tflops']:6.1f} TFLOP/s  windows: {r['flop_per_byte']:5.1f} FLOP/B "
+              f"{r['fill_tbs']:5.2f} TB/s L2->SMEM fill  (slab: {r['slab_flop_per_byte']:5.1f} FLOP/B "
+              f"{r['slab_fill_tbs']:5.2f} TB/s)  median SM clock {r['sm_mhz']} MHz")
     # one spot check of the result, so that a fast but wrong kernel cannot pass for a fast one
     ops.gemm_taps(As[0], B, outs[0], M=M, Kc=CI, taps=taps, block_n=160, image_map=(1, M, 0, 0, 1, M))
     rs = torch.arange(0, M, 4099, device=dev)
