@@ -79,4 +79,8 @@ __host__ __device__ constexpr int gemm_stage_bytes(int block_n) {
   return GEMM_BLOCK_M * GEMM_BLOCK_K * 2 + block_n * GEMM_BLOCK_K * 2;
 }
 
+// The persistent linear GEMM (gemm_linear.cu) for one-tap, plain-row-map calls with 16-bit output and residual, no row
+// bias and no split-K, at tile width bn (GEGLU: bn = 256 only). kp is the tap-GEMM's parameter block.
+int launch_gemm_linear(const pf_gemm_args* a, const GemmKernelParams& kp, int bn, cudaStream_t st);
+
 }  // namespace pf

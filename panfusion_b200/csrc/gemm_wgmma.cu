@@ -1,5 +1,6 @@
 // Tap-GEMM on Hopper: TMA (SWIZZLE_128B) -> shared-memory ring -> wgmma (m64 x BLOCK_N x k16 per warpgroup, fp32 in
-// registers) -> epilogue. One kernel serves nn.Linear and every 1x1 / 3x3 convolution of the UNet walk
+// registers) -> epilogue. One kernel serves every 3x3 convolution of the UNet walk and the GEMMs the persistent linear
+// kernel (gemm_linear.cu, routed to at the end of pf_gemm_taps) does not take: fp32 outputs, split-K, row bias
 // (reference call sites: models/pano/MVGenModel.py:85-295 through diffusers ResnetBlock2D / Transformer2DModel,
 //  models/modules/transformer.py:57-74,8-35). A convolution is a sum of `num_taps` GEMMs whose A operand is the
 // same channels-last image shifted by a constant row offset (zero-haloed "padded-flat" layout), so the im2col
@@ -833,6 +834,11 @@ extern "C" int pf_gemm_taps(const pf_gemm_args* a, void* stream) {
     PF_CHECK_LAUNCH("splitk_reduce_kernel");
     return PF_OK;
   }
+  // one-tap, plain-row-map calls with 16-bit output and 16-bit (or no) residual and no row bias: the persistent linear
+  // GEMM (gemm_linear.cu). It runs GEGLU at the 256-wide tile and every other epilogue at 64, 128 and 160 wide.
+  const bool plain16 = a->map_mode == 0 && a->out_dtype == a->dtype && (!a->residual || a->res_dtype == a->dtype);
+  if (a->num_taps == 1 && plain16 && !a->rowbias && (a->act == PF_ACT_GEGLU) == (bn == 256))
+    return launch_gemm_linear(a, kp, bn, st);
   // staged TMA-store epilogue: plain row map, 16-bit output, 16-bit (or no) residual, no GEGLU
   const bool epi_tma = a->map_mode == 0 && a->out_dtype == a->dtype && a->act != PF_ACT_GEGLU &&
                        (!a->residual || a->res_dtype == a->dtype) && bn != 256;

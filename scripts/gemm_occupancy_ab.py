@@ -11,10 +11,14 @@ alternate A, B, A, B, ... for `--rounds` rounds, each in a fresh process:
 2. `bench.py --gpus 1 --steps 20 --warmup 5 --skip-cpu --skip-image --dump-outputs <tmp>` for both builds, and a byte
    comparison of the dumped latents of build A and build B.
 
+Each child also hashes (sha256) the first output buffer of every shape after its timed launches, from inputs seeded per
+shape; the report says per shape whether build A's output equals build B's byte for byte.
+
 Prints min / median / max per shape and build, the card's name and power limit (read-only nvidia-smi query), and one
 JSON line with everything. Exits non-zero without a GPU. Nothing is written inside the repository.
 """
 import argparse
+import io
 import json
 import os
 import statistics
@@ -22,6 +26,8 @@ import subprocess
 import sys
 import tempfile
 from pathlib import Path
+
+import numpy as np
 
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
@@ -38,10 +44,13 @@ SHAPES = {
     "conv3x3_512_4x64x64": ("conv", (4, 64, 64, 512, 512)),         # 128-wide direct stores (VAE decoder width)
     "conv3x3_320to64_16x64x64": ("conv", (16, 64, 64, 320, 64)),    # 64-wide direct stores (conv_out's padded tile)
     "lin_320_320": ("lin", (T64, 320, 320), ("stats",)),            # proj_in / to_out
+    "lin_320_320_ln": ("lin", (T64, 320, 320), ("ln",)),            # cross-attention q behind a folded LayerNorm
     "lin_320_960_ln": ("lin", (T64, 320, 960), ("ln",)),            # fused q|k|v behind a folded LayerNorm
     "lin_1600_320_res_stats": ("lin", (T64, 1600, 320), ("res", "stats")),  # Transformer tail
     "lin_320_2560_geglu": ("lin", (T64, 320, 2560), ("ln", "geglu")),
     "lin_640_640": ("lin", (T32, 640, 640), ("stats",)),
+    "lin_320_640_shortcut": ("lin", (T32, 320, 640), ()),          # resnet 1x1 shortcut
+    "lin_1280_10240_geglu": ("lin", (T16, 1280, 10240), ("ln", "geglu")),  # GEGLU at the 16x16 level
     "lin_640_1920_ln": ("lin", (T32, 640, 1920), ("ln",)),
     "lin_1024_1024_res": ("lin", (T64 // 4, 1024, 1024), ("res",)),  # 128-wide TMA stores (text-encoder width)
     "lin_320_64": ("lin", (T64, 320, 64), ()),                      # 64-wide TMA stores
@@ -65,6 +74,8 @@ def nvidia_smi_line():
 
 # ------------------------------------------------ child: time the shapes with the library PF_LIB_PATH names
 def child(names):
+    import hashlib
+
     import torch
     from bench import ClockSampler
     from panfusion_b200 import _lib, ops
@@ -104,7 +115,7 @@ def child(names):
         As = [torch.randn(m, ci, device=dev).to(bf) for _ in range(sets)]
         outs = [torch.empty(n * h * w, co, dtype=bf, device=dev) for _ in range(sets)]
         return [(lambda a=a, o=o: ops.gemm_taps(a, wgt, o, M=m, Kc=ci, taps=taps3x3(wp), image_map=(hp, wp, 1, 1, h, w)))
-                for a, o in zip(As, outs)]
+                for a, o in zip(As, outs)], outs[0]
 
     def lin_fns(m, k, n, flags):
         geglu = "geglu" in flags
@@ -125,17 +136,20 @@ def child(names):
         if "stats" in flags:
             kw["row_stats"] = True
         ress = [torch.randn(m, n_out, device=dev).to(bf) for _ in range(sets)] if "res" in flags else [None] * sets
-        return [(lambda a=a, o=o, r=r: ops.gemm_taps(a, wgt, o, residual=r, **kw)) for a, o, r in zip(As, outs, ress)]
+        return [(lambda a=a, o=o, r=r: ops.gemm_taps(a, wgt, o, residual=r, **kw)) for a, o, r in zip(As, outs, ress)], outs[0]
 
-    res = {}
+    res, digest = {}, {}
     with ClockSampler(0) as clk:
         for name in names:
             kind, dims = SHAPES[name][0], SHAPES[name][1]
-            fns = conv_fns(*dims) if kind == "conv" else lin_fns(*dims, SHAPES[name][2])
+            torch.manual_seed(0)  # the same operands for both builds
+            fns, out0 = conv_fns(*dims) if kind == "conv" else lin_fns(*dims, SHAPES[name][2])
             res[name] = round(timeit(fns) * 1e3, 2)  # us per launch
-            del fns
+            torch.cuda.synchronize()
+            digest[name] = hashlib.sha256(out0.view(torch.uint8).cpu().numpy().tobytes()).hexdigest()
+            del fns, out0
             torch.cuda.empty_cache()
-    print(json.dumps(dict(us=res, sm_mhz=clk.summary()["sm_mhz"])))
+    print(json.dumps(dict(us=res, sha256=digest, sm_mhz=clk.summary()["sm_mhz"])))
 
 
 # ------------------------------------------------ parent: alternate the two builds
@@ -185,19 +199,28 @@ def main():
     me = str(Path(__file__).resolve())
     us = [{n: [] for n in args.shapes} for _ in libs]
     mhz = [[], []]
+    digests = [[], []]
     for _ in range(args.rounds):
         for i, lib in enumerate(libs):
             r = run_child(lib, [me, "--child", "--shapes", *args.shapes], "shape timing")
             for n, v in r["us"].items():
                 us[i][n].append(v)
             mhz[i].append(r["sm_mhz"])
+            digests[i].append(r["sha256"])
     print(f"\nus per launch, min / median / max over {args.rounds} alternated processes "
           f"(median SM clock A {mhz[0]} MHz, B {mhz[1]} MHz)")
-    print(f"{'shape':28s} {'A min':>8s} {'A med':>8s} {'A max':>8s}   {'B min':>8s} {'B med':>8s} {'B max':>8s}   B/A time   B TFLOP/s")
+    print(f"{'shape':28s} {'A min':>8s} {'A med':>8s} {'A max':>8s}   {'B min':>8s} {'B med':>8s} {'B max':>8s}   B/A time"
+          f"   B TFLOP/s   A == B output")
+    same = {}
     for n in args.shapes:
         ma, mb = statistics.median(us[0][n]), statistics.median(us[1][n])
-        print(f"{n:28s} {mmm(us[0][n])}   {mmm(us[1][n])}   {mb / ma:8.3f}   {shape_flops(n) / mb / 1e6:8.1f}")
-    out = dict(gpu=torch.cuda.get_device_name(0), smi=smi, libs=[str(p) for p in libs], us=us, sm_mhz=mhz)
+        # each build must repeat itself; then the two builds' outputs are compared byte for byte
+        rep = all(d[n] == digests[i][0][n] for i in range(2) for d in digests[i])
+        same[n] = "yes" if rep and digests[0][0][n] == digests[1][0][n] else ("NO" if rep else "NOT REPEATABLE")
+        print(f"{n:28s} {mmm(us[0][n])}   {mmm(us[1][n])}   {mb / ma:8.3f}   {shape_flops(n) / mb / 1e6:8.1f}   "
+              f"{same[n]:>13s}")
+    out = dict(gpu=torch.cuda.get_device_name(0), smi=smi, libs=[str(p) for p in libs], us=us, sm_mhz=mhz,
+               outputs_identical=same)
 
     if not args.skip_bench:
         steps = [[], []]
@@ -214,13 +237,24 @@ def main():
                     dumps[i].append({f.name: f.read_bytes() for f in sorted(d.glob("*.npy"))})
             same_build = all(d == dumps[i][0] for i in range(2) for d in dumps[i])
             same_ab = dumps[0][0] == dumps[1][0] and len(dumps[0][0]) > 0
+            # how far B's latents lie from A's, relative to max|latent| of A
+            rel = {}
+            for f, ba in dumps[0][0].items():
+                if f in dumps[1][0]:
+                    xa = np.load(io.BytesIO(ba)).astype(np.float64)
+                    xb = np.load(io.BytesIO(dumps[1][0][f])).astype(np.float64)
+                    d = np.abs(xb - xa) / max(np.abs(xa).max(), 1e-30)
+                    rel[f] = dict(max=float(d.max()), mean=float(d.mean()))
         print(f"\nbench.py steps/s (C2, 1 GPU, 20 steps): A {mmm(steps[0])} (SM MHz {clocks[0]})\n"
               f"{'':39s}B {mmm(steps[1])} (SM MHz {clocks[1]})")
+        for f, r in rel.items():
+            print(f"--dump-outputs {f}: |B - A| / max|A| max {r['max']:.3g}, mean {r['mean']:.3g}")
         gain = statistics.median(steps[1]) / statistics.median(steps[0]) - 1
         apart = min(steps[1]) > max(steps[0]) or max(steps[1]) < min(steps[0])
         print(f"B vs A: {gain * 100:+.2f} % median, ranges {'do not overlap' if apart else 'OVERLAP'}; "
               f"--dump-outputs: each build identical across its runs: {same_build}; A and B byte-identical: {same_ab}")
-        out.update(steps_per_s=steps, bench_sm_mhz=clocks, dumps_identical=same_ab, dumps_repeatable=same_build)
+        out.update(steps_per_s=steps, bench_sm_mhz=clocks, dumps_identical=same_ab, dumps_repeatable=same_build,
+                   dumps_rel_diff=rel)
     print(json.dumps(out))
 
 

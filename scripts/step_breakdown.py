@@ -8,8 +8,12 @@ of every kernel by family. The tap-GEMM is split into classes by its template ar
 <BLOCK_N, STAGES, CTAS, BF16, EPI_TMA>:
   conv (direct store)   EPI_TMA = false, two CTAs per SM: the convolutions (and fp32-output linears)
   split-K partials      EPI_TMA = false, one CTA per SM, BLOCK_N < 256: the deep-K convolutions of small images
-  linear (TMA store)    EPI_TMA = true: the linear layers
+  linear (TMA store)    EPI_TMA = true: plain-row-map calls the persistent linear GEMM does not take (multi-tap, row bias)
   GEGLU 256-wide        BLOCK_N = 256
+The persistent linear GEMM, gemm_linear_kernel<BLOCK_N, STAGES, GEGLU, BF16>, which runs the one-tap, plain-row-map
+calls with 16-bit output (the linear layers and 1x1 shortcuts), is split by width:
+  linear GEMM           the 64-, 128- and 160-wide tiles
+  linear GEMM GEGLU     the 256-wide GEGLU tile
 The sum is kernel time only: launch gaps, which a CUDA-graph step of bench.py mostly removes, are not counted.
 Profile in a run of its own; take step rates from bench.py. Prints the card's name and power limit.
 """
@@ -27,9 +31,13 @@ import torch  # noqa: E402
 import bench  # noqa: E402
 
 GEMM_RE = re.compile(r"gemm_taps_kernel<(\d+),\s*(\d+),\s*(\d+),\s*(\w+),\s*(\w+)>")
+LINEAR_RE = re.compile(r"gemm_linear_kernel<(\d+),\s*(\d+),\s*(\w+),\s*(\w+)>")
 
 
 def family(name: str) -> str:
+    m = LINEAR_RE.search(name)
+    if m:
+        return "linear GEMM GEGLU 256-wide" if m.group(3) == "true" else "linear GEMM 64/128/160-wide"
     m = GEMM_RE.search(name)
     if m:
         bn, _, ctas, _, epi_tma = m.groups()
