@@ -106,10 +106,12 @@ int pf_p2e(const void* src, void* dst, uint8_t* mask, int dtype, int B, int C, i
  *   map_mode 0: row(m) = m, group(m) = m / rows_per_group
  *   map_mode 1: m -> (img, i, j) with i = (m / Wm) % Hm, j = m % Wm; valid iff i0 <= i < i0+Hout and
  *               j0 <= j < j0+Wout; row(m) = (img*Hout + i-i0)*Wout + (j-j0); group(m) = img
- * act: PF_ACT_GEGLU expects B (and bias) packed so that every block_n-wide column tile holds block_n/2 value
- * columns followed by their block_n/2 gate columns; it writes N/2 output columns. PF_ACT_GELU is erf-GELU (F.gelu),
+ * act: PF_ACT_GEGLU expects B (and bias) packed so that every 256-wide column tile holds 128 value columns followed
+ * by their 128 gate columns; it writes N/2 output columns. GEGLU runs only at block_n = 256 and needs one tap,
+ * map_mode 0, a 16-bit output, k_splits <= 1 and no residual or rowbias. PF_ACT_GELU is erf-GELU (F.gelu),
  * PF_ACT_QUICK_GELU is CLIP's x * sigmoid(1.702 x); both apply wherever PF_ACT_SILU does (epilogues, split-K reduce).
- * Constraints: Kc % 64 == 0, N % block_n == 0, block_n in {64,128,160,256}, a_ld/b_ld % 8 == 0.
+ * Constraints: Kc % 64 == 0, N % block_n == 0, block_n in {64,128,160} (256 only with GEGLU), a_ld/b_ld % 8 == 0.
+ * A call outside the contract returns PF_ERR_INVALID with a message before any CUDA call.
  * Alignment (checked, PF_ERR_INVALID otherwise): A, B, out, residual, rowbias, splitk_ws and ln_stats 16 bytes;
  * row_stats_out 8 bytes; out_ld, res_ld % 8 == 0 and rowbias_ld % 4 == 0 (elements), so every row stays aligned.
  * ------------------------------------------------------------------------------------------------ */
@@ -125,7 +127,7 @@ typedef struct pf_gemm_args {
   int32_t dtype; /* PF_F16 | PF_BF16 (A and B) */
   int32_t M, N, Kc, num_taps;
   int32_t tap_off[PF_MAX_TAPS];
-  int32_t block_n; /* 0 = auto */
+  int32_t block_n; /* 0 = auto (pf_gemm_pick_block_n), else 64, 128, 160, or 256 with GEGLU */
   void* out;
   int32_t out_ld;
   int32_t out_dtype; /* PF_F32 or same as dtype */
@@ -151,7 +153,8 @@ typedef struct pf_gemm_args {
    *     ln_colsum[n] = sum_k W'[n,k] (of the 16-bit rounded W'), bias[n] = sum_k beta[k] W[n,k] + b[n]; the epilogue applies
    *     acc <- rstd[m] * (acc - mean[m] * ln_colsum[n]) with mean / rstd from ln_stats[m][ln_slots][2] over K = Kc*num_taps
    *     elements, biased variance, eps = ln_eps — algebraically LayerNorm(A) W^T + b with the normalised tensor never
-   *     stored. Supported with the plain row map and 16-bit output, or with the GEGLU epilogue. */
+   *     stored. Both sides need one tap, no rowbias, no split-K, the plain row map and a 16-bit output; the consumer
+   *     may also run the GEGLU epilogue. */
   /* map_mode 1 with an output SCATTER (0 / 1 = off): the valid pixel (i, j) of image img is written to row
    *   ((img*Hout + i-i0)*out_sy + out_a) * (Wout*out_sx) + (j-j0)*out_sx + out_b
    * i.e. phase (out_a, out_b) of an image up-sampled by (out_sy, out_sx). Upsample2D's nearest-x2 followed by a 3x3
@@ -167,11 +170,12 @@ typedef struct pf_gemm_args {
 
 int pf_gemm_taps(const pf_gemm_args* args, void* stream);
 /* number of column slots a producer with these args writes per row of row_stats_out: 2 per column tile, and a producer's
- * tile width is a function of N alone (requests / tuning are ignored), so the statistics are bit-identical for any M */
+ * tile width is a function of N alone (block_n requests are ignored), so the statistics are bit-identical for any M */
 int pf_gemm_row_stats_slots(const pf_gemm_args* args);
 /* suggested k_splits for this problem (1 = do not split); only M, N, Kc, num_taps, act, map_mode, dtypes are read */
 int pf_gemm_splitk_plan(const pf_gemm_args* args);
-/* block_n the auto-tuner would pick for this N (used by the host-side weight packer for GEGLU) */
+/* block_n that block_n = 0 selects for this N: 160, 128 or 64 (the widest that divides N), for GEGLU 256; 0 if none
+ * divides N (used by the host-side weight packer for GEGLU) */
 int pf_gemm_pick_block_n(int N, int act);
 
 /* ------------------------------------------------------------------------------------------------

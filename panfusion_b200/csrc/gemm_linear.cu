@@ -44,6 +44,31 @@ __host__ __device__ constexpr int lin_smem_bytes(int block_n, int stages, bool g
          2 * GEMM_BLOCK_M * 8 /*two slots of LayerNorm coefficients*/ + (2 * stages + 6) * 8;
 }
 
+// mean / rstd of one row from the producer's partial sums, as the two epilogue coefficients of the LayerNorm fold:
+// acc <- acc * a + colsum[n] * b with a = rstd, b = -mean * rstd
+__device__ __forceinline__ void ln_row_coeffs(const GemmKernelParams& p, long long m, float& a, float& b) {
+  // slots come in pairs (two per column tile): 16-byte loads, four of them in flight, summed in slot order
+  const float4* st = reinterpret_cast<const float4*>(p.ln_stats) + m * (p.ln_slots >> 1);
+  const int pairs = p.ln_slots >> 1;
+  float s = 0.f, q = 0.f;
+  for (int i0 = 0; i0 < pairs; i0 += 4) {
+    float4 v[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) v[u] = i0 + u < pairs ? __ldg(st + i0 + u) : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      s += v[u].x;
+      q += v[u].y;
+      s += v[u].z;
+      q += v[u].w;
+    }
+  }
+  const float mean = s * p.ln_inv_k;
+  const float var = fmaxf(q * p.ln_inv_k - mean * mean, 0.f);
+  a = rsqrtf(var + p.ln_eps);
+  b = -mean * a;
+}
+
 __device__ __forceinline__ void setmaxnreg_inc232() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory"); }
 __device__ __forceinline__ void setmaxnreg_dec40() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory"); }
 

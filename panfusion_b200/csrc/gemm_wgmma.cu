@@ -1,29 +1,29 @@
 // Tap-GEMM on Hopper: TMA (SWIZZLE_128B) -> shared-memory ring -> wgmma (m64 x BLOCK_N x k16 per warpgroup, fp32 in
-// registers) -> epilogue. One kernel serves every 3x3 convolution of the UNet walk and the GEMMs the persistent linear
-// kernel (gemm_linear.cu, routed to at the end of pf_gemm_taps) does not take: fp32 outputs, split-K, row bias
-// (reference call sites: models/pano/MVGenModel.py:85-295 through diffusers ResnetBlock2D / Transformer2DModel,
-//  models/modules/transformer.py:57-74,8-35). A convolution is a sum of `num_taps` GEMMs whose A operand is the
-// same channels-last image shifted by a constant row offset (zero-haloed "padded-flat" layout), so the im2col
-// matrix is never formed. Taps whose offsets lie within GEMM_WIN_SPAN (8) rows of each other (the three taps of a 3x3
-// kernel row) read one A window of 128 + 8 rows, fetched once per 64-channel slab with one 2-D TMA box, and each tap's
-// wgmma A operand starts 0..8 rows into it; only the B box is fetched per tap. A 3x3 convolution's tile so reads each
-// A row 3 times per channel slab from L2 instead of 9. A GEMM whose taps are all further apart (linears, 1x1
-// convolutions) runs the plain slab ring: one A box and one B box per K-slab behind one barrier.
+// registers) -> epilogue. It runs every pf_gemm_taps call the persistent linear GEMM (gemm_linear.cu) does not take:
+// the 3x3 convolutions and Upsample2D / Downsample2D phase convolutions of the UNet walk, fp32 outputs, row bias and
+// split-K (reference call sites: models/pano/MVGenModel.py:85-295 through diffusers ResnetBlock2D /
+// Transformer2DModel). A convolution is a sum of `num_taps` GEMMs whose A operand is the same channels-last image
+// shifted by a constant row offset (zero-haloed "padded-flat" layout), so the im2col matrix is never formed. Taps whose
+// offsets lie within GEMM_WIN_SPAN (8) rows of each other (the three taps of a 3x3 kernel row) read one A window of
+// 128 + 8 rows, fetched once per 64-channel slab with one 2-D TMA box, and each tap's wgmma A operand starts 0..8 rows
+// into it; only the B box is fetched per tap. A 3x3 convolution's tile so reads each A row 3 times per channel slab
+// from L2 instead of 9. A GEMM whose taps are all further apart (1x1 convolutions, single-tap GEMMs) runs the plain
+// slab ring: one A box and one B box per K-slab behind one barrier.
 //
 // 256 threads: warps 0..3 and 4..7 = two warpgroups, each owning 64 of the 128 tile rows through the main loop.
 // There is no producer warp: thread 0 fills the ring before the loop, and the leader of whichever warpgroup releases
-// a slot last issues the slot's next TMA loads, so no MMA-issuing warp ever blocks on the other warpgroup. After the last K-slab the accumulators are written to shared memory (over the now idle operand
-// ring) and all 256 threads run the epilogue with two threads per tile row (even / odd 16-column chunks): bias / LayerNorm fold / per-image row bias / SiLU / GELU / GEGLU / residual,
-// then either (EPI_TMA) swizzled [128][32] sub-tiles streamed out with TMA tile stores through two staging buffers
-// behind the accumulators, or direct stores through the halo-dropping row map (convolutions, fp32 outputs, GEGLU),
-// or raw fp32 split-K partials.
+// a slot last issues the slot's next TMA loads, so no MMA-issuing warp ever blocks on the other warpgroup. After the
+// last K-slab the accumulators are written to shared memory (over the now idle operand ring) and all 256 threads run
+// the epilogue with two threads per tile row (even / odd 16-column chunks). It has two forms: raw fp32 split-K
+// partials, or bias / per-image row bias / SiLU / GELU / QuickGELU / residual stored directly through the
+// halo-dropping row map.
 //
 // Instantiations with a short ring (CTAS = 2) run TWO CTAs per SM (at most 128 registers per thread and 113 KB of
 // shared memory per CTA): a tile has no overlap of its own between ring fill, main loop, accumulator dump and
 // epilogue, so the tensor pipe is kept busy by the other CTA's main loop while one CTA fills or drains. A ninth
 // (producer) warp would rule that out: registers are granted to whole warps, nine warps would leave two CTAs 96
-// registers per thread, and the 160-wide tile alone holds 80 accumulators. The 256-wide GEGLU tile (128 accumulators,
-// 133 KB accumulator dump) and split-K, which is planned at about one CTA per SM, keep a long ring and CTAS = 1.
+// registers per thread, and the 160-wide tile alone holds 80 accumulators. Split-K, which is planned at about one CTA
+// per SM, keeps a long ring and CTAS = 1.
 #include <stdlib.h>
 
 #include "gemm_common.cuh"
@@ -33,45 +33,38 @@ namespace pf {
 
 constexpr int GEMM_THREADS = 256;
 
-constexpr int GEMM_SUB_BYTES = GEMM_BLOCK_M * 64;  // one [128][32] 16-bit sub-tile of the TMA-store epilogue, SWIZZLE_64B
 // an SM has 228 KB of shared memory and every resident CTA reserves 1 KB of it
 constexpr int GEMM_SMEM_CORESIDENT = 228 * 1024 / 2 - 1024;
 
 __host__ __device__ constexpr int gemm_acc_ld(int block_n) { return block_n + 4; }  // floats; +4: conflict-free rows
-// accumulator dump, rounded up to the 1024 bytes that keep the staging buffers behind it swizzle-aligned
-__host__ __device__ constexpr int gemm_acc_bytes(int block_n) {
-  return (GEMM_BLOCK_M * gemm_acc_ld(block_n) * 4 + 1023) / 1024 * 1024;
-}
-// the operand ring; after the main loop the same bytes hold the accumulators and (EPI_TMA) two staging sub-tiles
-__host__ __device__ constexpr int gemm_ring_bytes(int block_n, int stages, bool epi_tma) {
+// the operand ring; after the main loop the same bytes hold the [128][acc_ld] fp32 accumulators
+__host__ __device__ constexpr int gemm_ring_bytes(int block_n, int stages) {
   const int ring = stages * gemm_stage_bytes(block_n);
-  const int epi = gemm_acc_bytes(block_n) + (epi_tma ? 2 * GEMM_SUB_BYTES : 0);
-  return ((ring > epi ? ring : epi) + 1023) / 1024 * 1024;
+  const int acc = GEMM_BLOCK_M * gemm_acc_ld(block_n) * 4;
+  return ((ring > acc ? ring : acc) + 1023) / 1024 * 1024;
 }
 // full barrier (8 bytes) and release counter (4 bytes) per A slot and per B slot (at most STAGES of each), rounded up
 // to keep s_bias 16-byte aligned
 __host__ __device__ constexpr int gemm_bar_bytes(int stages) { return (2 * stages * 12 + 15) / 16 * 16; }
-__host__ __device__ constexpr int gemm_smem_bytes(int block_n, int stages, bool epi_tma) {
-  return gemm_ring_bytes(block_n, stages, epi_tma) + gemm_bar_bytes(stages) +
-         2 * block_n * 4 /*bias row + LayerNorm column sums*/;
+__host__ __device__ constexpr int gemm_smem_bytes(int block_n, int stages) {
+  return gemm_ring_bytes(block_n, stages) + gemm_bar_bytes(stages) + block_n * 4 /*bias row*/;
 }
 
-template <int BLOCK_N, int STAGES, int CTAS, bool BF16, bool EPI_TMA>
+template <int BLOCK_N, int STAGES, int CTAS, bool BF16>
 __global__ void __launch_bounds__(GEMM_THREADS, CTAS)
 gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmC, const GemmKernelParams p) {
+                 const GemmKernelParams p) {
   constexpr int B_BYTES = BLOCK_N * GEMM_BLOCK_K * 2;
-  constexpr int RING_BYTES = gemm_ring_bytes(BLOCK_N, STAGES, EPI_TMA);
+  constexpr int RING_BYTES = gemm_ring_bytes(BLOCK_N, STAGES);
   constexpr int ACC_LD = gemm_acc_ld(BLOCK_N);
   constexpr int NCH = BLOCK_N / 16;
   constexpr int NACC = BLOCK_N / 2;  // fp32 accumulators per thread of an m64 x BLOCK_N warpgroup tile
-  static_assert(BLOCK_N % 32 == 0 && BLOCK_N <= 256, "tile width");
+  static_assert(BLOCK_N % 32 == 0 && BLOCK_N <= 160, "tile width");
 
   // 1024-byte alignment (128 B swizzle atoms) is requested on the declaration; verified once, never padded for
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   float* sacc = reinterpret_cast<float*>(smem);  // [128][ACC_LD] fp32, over the ring once the main loop is done
-  uint8_t* staging = smem + gemm_acc_bytes(BLOCK_N);  // EPI_TMA: two [128][32] 16-bit sub-tiles, also inside the ring
   // the ring: p.a_slots A windows, then STAGES B boxes (1024-byte multiples, so every slot is swizzle-aligned)
   const int a_bytes = p.a_rows * (GEMM_BLOCK_K * 2);
   uint8_t* const b_ring = smem + p.a_slots * a_bytes;
@@ -80,7 +73,6 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint32_t* a_rel = reinterpret_cast<uint32_t*>(b_full + STAGES);  // per slot: releases by the two warpgroups
   uint32_t* b_rel = a_rel + STAGES;
   float* s_bias = reinterpret_cast<float*>(smem + RING_BYTES + gemm_bar_bytes(STAGES));  // [BLOCK_N]
-  float* s_cs = s_bias + BLOCK_N;  // [BLOCK_N] LayerNorm column sums
 
   const int et = threadIdx.x;  // 0..255
   const int lane = et & 31;
@@ -108,7 +100,6 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       mbar_init(&b_full[s], 1);
       a_rel[s] = b_rel[s] = 0u;
     }
-    if constexpr (EPI_TMA) tma_prefetch_desc(&tmC);
     fence_barrier_init();
   }
   __syncthreads();
@@ -161,7 +152,6 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
   // ------------------------------ main loop ------------------------------
   if (p.bias && et < BLOCK_N) s_bias[et] = __ldg(p.bias + n0 + et);
-  if (p.ln_stats && et < BLOCK_N) s_cs[et] = __ldg(p.ln_colsum + n0 + et);
   {
     float acc[NACC];
 #pragma unroll
@@ -284,9 +274,6 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   } else if (p.rowbias) {
     group = m / p.rows_per_group;
   }
-  if (!valid) group = 0;  // rows past M are computed (and clipped by the TMA store): keep their table reads in bounds
-  float ln_a = 1.f, ln_b = 0.f;
-  if (p.ln_stats && m < p.M) ln_row_coeffs(p, m, ln_a, ln_b);
   const float* rb_base = p.rowbias ? p.rowbias + (long long)group * p.rowbias_ld + n0 : nullptr;
   auto load16 = [&](int c, float (&o)[16]) {
 #pragma unroll
@@ -312,132 +299,8 @@ gemm_taps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int e = 0; e < 4; ++e) dst[e] = make_float4(o[4 * e], o[4 * e + 1], o[4 * e + 2], o[4 * e + 3]);
       }
     }
-  } else if constexpr (EPI_TMA) {
-    // The tile leaves in [128][32] sub-tiles: the two threads of a row fill one 16-column chunk each, thread 0 hands the
-    // sub-tile to a TMA store, and the next sub-tile goes to the other staging buffer while that store reads this one.
-    static_assert(NCH % 2 == 0, "a sub-tile is one chunk of each of a row's two threads");
-    const uint32_t sw = uint32_t((row >> 1) & 3);  // SWIZZLE_64B: 16-byte chunk index ^= address bits [7,9)
-    float st_s = 0.f, st_q = 0.f;                   // row statistics of this thread's chunks = slot `half`
-    // rows past M are computed and clipped by the TMA store: they read no residual
-    const uint16_t* res_row =
-        p.residual && m < p.M ? static_cast<const uint16_t*>(p.residual) + (long long)m * p.res_ld + n0 : nullptr;
-#pragma unroll 1
-    for (int ci = half; ci < NCH; ci += 2) {
-      const int c = ci * 16;
-      uint4 r0 = make_uint4(0u, 0u, 0u, 0u), r1 = r0;
-      if (res_row) {
-        r0 = __ldg(reinterpret_cast<const uint4*>(res_row + c));
-        r1 = __ldg(reinterpret_cast<const uint4*>(res_row + c) + 1);
-      }
-      float o[16];
-      load16(c, o);
-      if (p.ln_stats) {
-#pragma unroll
-        for (int e = 0; e < 16; ++e) o[e] = fmaf(o[e], ln_a, s_cs[c + e] * ln_b);
-      }
-      if (p.bias) {
-#pragma unroll
-        for (int e = 0; e < 16; ++e) o[e] += s_bias[c + e];
-      }
-      if (rb_base) {
-#pragma unroll
-        for (int e = 0; e < 16; ++e) o[e] += __ldg(rb_base + c + e);
-      }
-      if (p.act == PF_ACT_SILU) {
-#pragma unroll
-        for (int e = 0; e < 16; ++e) o[e] = silu_f(o[e]);
-      } else if (p.act == PF_ACT_GELU) {
-#pragma unroll
-        for (int e = 0; e < 16; ++e) o[e] = gelu_erf_f(o[e]);
-      } else if (p.act == PF_ACT_QUICK_GELU) {
-#pragma unroll
-        for (int e = 0; e < 16; ++e) o[e] = quick_gelu_f(o[e]);
-      }
-      const int sub = c >> 5;
-      uint8_t* sbuf = staging + (sub & 1) * GEMM_SUB_BYTES;
-      uint8_t* srow = sbuf + row * 64;
-      const uint32_t q0 = uint32_t((c >> 4) & 1) * 2;  // first 16-byte chunk of this 16-column group in the 64 B row
-      uint4* s0 = reinterpret_cast<uint4*>(srow + (((q0 + 0) ^ sw) << 4));
-      uint4* s1 = reinterpret_cast<uint4*>(srow + (((q0 + 1) ^ sw) << 4));
-      if (p.residual) {  // rows past M add the zeros above
-        float2 f;
-        f = unpack2<BF16>(r0.x); o[0] += f.x; o[1] += f.y;
-        f = unpack2<BF16>(r0.y); o[2] += f.x; o[3] += f.y;
-        f = unpack2<BF16>(r0.z); o[4] += f.x; o[5] += f.y;
-        f = unpack2<BF16>(r0.w); o[6] += f.x; o[7] += f.y;
-        f = unpack2<BF16>(r1.x); o[8] += f.x; o[9] += f.y;
-        f = unpack2<BF16>(r1.y); o[10] += f.x; o[11] += f.y;
-        f = unpack2<BF16>(r1.z); o[12] += f.x; o[13] += f.y;
-        f = unpack2<BF16>(r1.w); o[14] += f.x; o[15] += f.y;
-      }
-      if (p.row_stats) {
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          st_s += o[e];
-          st_q = fmaf(o[e], o[e], st_q);
-        }
-      }
-      *s0 = make_uint4(pack2<BF16>(o[0], o[1]), pack2<BF16>(o[2], o[3]), pack2<BF16>(o[4], o[5]),
-                       pack2<BF16>(o[6], o[7]));
-      *s1 = make_uint4(pack2<BF16>(o[8], o[9]), pack2<BF16>(o[10], o[11]), pack2<BF16>(o[12], o[13]),
-                       pack2<BF16>(o[14], o[15]));
-      fence_proxy_async_smem();  // generic-proxy writes -> visible to the TMA store
-      // the previous sub-tile's store has read its buffer before anyone passes this barrier and refills it
-      if (et == 0) tma_store_wait_read();
-      named_bar_sync(1, GEMM_THREADS);
-      if (et == 0) {
-        tma_store_2d(&tmC, sbuf, n0 + sub * 32, m0);
-        tma_store_commit();
-      }
-    }
-    if (p.row_stats && m < p.M)
-      reinterpret_cast<float2*>(p.row_stats)[(long long)m * p.stat_slots + n_tile * 2 + half] = make_float2(st_s, st_q);
-    if (et == 0) tma_store_wait_read();  // shared memory must outlive the last store's reads
-  } else if (p.act == PF_ACT_GEGLU) {
-    constexpr int HALF_N = BLOCK_N / 2;
-    const int on0 = n_tile * HALF_N;
-    if constexpr (HALF_N % 16 == 0) {
-#pragma unroll 1
-      for (int c = half * 16; c < HALF_N; c += 32) {
-        if (!valid) break;
-        float va[16], vg[16], o[16], ba[16], bg[16];
-        load16(c, va);
-        load16(HALF_N + c, vg);
-        if (p.bias) {  // HALF_N and c are multiples of 16: 128-bit shared-memory loads
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            *reinterpret_cast<float4*>(ba + 4 * e) = *reinterpret_cast<const float4*>(s_bias + c + 4 * e);
-            *reinterpret_cast<float4*>(bg + 4 * e) = *reinterpret_cast<const float4*>(s_bias + HALF_N + c + 4 * e);
-          }
-        } else {
-#pragma unroll
-          for (int e = 0; e < 16; ++e) ba[e] = bg[e] = 0.f;
-        }
-        if (p.ln_stats) {
-#pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            va[e] = fmaf(va[e], ln_a, s_cs[c + e] * ln_b);
-            vg[e] = fmaf(vg[e], ln_a, s_cs[HALF_N + c + e] * ln_b);
-          }
-        }
-#pragma unroll
-        for (int e = 0; e < 16; e += 2)
-          geglu_pair(va[e], va[e + 1], vg[e], vg[e + 1], ba[e], ba[e + 1], bg[e], bg[e + 1], o[e], o[e + 1]);
-        if (p.out_f32) {
-          float4* dst = reinterpret_cast<float4*>(static_cast<float*>(p.out) + orow * p.out_ld + on0 + c);
-#pragma unroll
-          for (int e = 0; e < 4; ++e) dst[e] = make_float4(o[4 * e], o[4 * e + 1], o[4 * e + 2], o[4 * e + 3]);
-        } else {
-          uint4* dst = reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.out) + orow * p.out_ld + on0 + c);
-          dst[0] = make_uint4(pack2<BF16>(o[0], o[1]), pack2<BF16>(o[2], o[3]), pack2<BF16>(o[4], o[5]),
-                              pack2<BF16>(o[6], o[7]));
-          dst[1] = make_uint4(pack2<BF16>(o[8], o[9]), pack2<BF16>(o[10], o[11]), pack2<BF16>(o[12], o[13]),
-                              pack2<BF16>(o[14], o[15]));
-        }
-      }
-    }
   } else if (valid) {
-    // direct stores (convolutions: halo-dropping row map; fp32 outputs)
+    // direct stores through the row map
 #pragma unroll 1
     for (int ci = half; ci < NCH; ci += 2) {
       const int c = ci * 16;
@@ -587,16 +450,16 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const GemmKernelPara
 }
 
 // CTAS: CTAs per SM the instantiation is built for (register cap of the build, shared-memory budget, checked below)
-template <int BLOCK_N, int STAGES, int CTAS, bool EPI_TMA>
+template <int BLOCK_N, int STAGES, int CTAS>
 static int launch_gemm(const pf_gemm_args* a, GemmKernelParams kp, cudaStream_t st) {
   // STAGES B boxes, and as many A windows as the rest of the ring holds (a slab ring: STAGES 128-row boxes)
-  const int a_slots = (gemm_ring_bytes(BLOCK_N, STAGES, EPI_TMA) - STAGES * BLOCK_N * GEMM_BLOCK_K * 2) /
+  const int a_slots = (gemm_ring_bytes(BLOCK_N, STAGES) - STAGES * BLOCK_N * GEMM_BLOCK_K * 2) /
                       (kp.a_rows * GEMM_BLOCK_K * 2);
   kp.a_slots = a_slots < STAGES ? a_slots : STAGES;
   // a window is refilled when the last tap of the window before it has retired: the ring needs two of them
-  static_assert(gemm_ring_bytes(BLOCK_N, STAGES, EPI_TMA) - STAGES * BLOCK_N * GEMM_BLOCK_K * 2 >= 2 * GEMM_WIN_BYTES,
+  static_assert(gemm_ring_bytes(BLOCK_N, STAGES) - STAGES * BLOCK_N * GEMM_BLOCK_K * 2 >= 2 * GEMM_WIN_BYTES,
                 "two A windows next to the B boxes");
-  CUtensorMap tmA, tmB, tmC;
+  CUtensorMap tmA, tmB;
   {
     uint64_t dims[2] = {(uint64_t)a->Kc, (uint64_t)a->a_rows};
     uint64_t str[1] = {(uint64_t)a->a_ld * 2};
@@ -611,22 +474,13 @@ static int launch_gemm(const pf_gemm_args* a, GemmKernelParams kp, cudaStream_t 
     int rc = make_tmap(&tmB, a->dtype, 2, a->B, dims, str, box, 128);
     if (rc) return rc;
   }
-  tmC = tmA;
-  if constexpr (EPI_TMA) {
-    uint64_t dims[2] = {(uint64_t)a->N, (uint64_t)a->M};
-    uint32_t box[2] = {32, GEMM_BLOCK_M};
-    uint64_t str[1] = {(uint64_t)a->out_ld * 2};
-    int rc = make_tmap(&tmC, a->dtype, 2, a->out, dims, str, box, 64);
-    if (rc) return rc;
-  }
-  constexpr int SMEM = gemm_smem_bytes(BLOCK_N, STAGES, EPI_TMA);
+  constexpr int SMEM = gemm_smem_bytes(BLOCK_N, STAGES);
   static_assert(SMEM <= 227 * 1024, "shared memory budget of one H100 CTA");
   static_assert(CTAS == 1 || SMEM <= GEMM_SMEM_CORESIDENT, "two CTAs per SM: 113 KB of shared memory each");
   const int m_tiles = (a->M + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M;
   const dim3 grid(m_tiles * (a->N / BLOCK_N), kp.k_splits > 1 ? kp.k_splits : 1);
   const int bf = a->dtype == PF_BF16;
-  auto kern = bf ? gemm_taps_kernel<BLOCK_N, STAGES, CTAS, true, EPI_TMA>
-                 : gemm_taps_kernel<BLOCK_N, STAGES, CTAS, false, EPI_TMA>;
+  auto kern = bf ? gemm_taps_kernel<BLOCK_N, STAGES, CTAS, true> : gemm_taps_kernel<BLOCK_N, STAGES, CTAS, false>;
   static bool attr_set[2] = {false, false};  // per dtype: the two kernels share this function's statics
   if (!attr_set[bf]) {
     int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM),
@@ -638,26 +492,21 @@ static int launch_gemm(const pf_gemm_args* a, GemmKernelParams kp, cudaStream_t 
                     "cudaOccupancyMaxActiveBlocksPerMultiprocessor(gemm)");
     if (rc) return rc;
     if (resident < CTAS) {
-      set_error("gemm_taps_kernel<%d, %d, %s>: %d CTA(s) per SM fit, built for %d", BLOCK_N, STAGES,
-                EPI_TMA ? "tma" : "direct", resident, CTAS);
+      set_error("gemm_taps_kernel<%d, %d>: %d CTA(s) per SM fit, built for %d", BLOCK_N, STAGES, resident, CTAS);
       return PF_ERR_UNSUPPORTED;
     }
     attr_set[bf] = true;
   }
-  kern<<<grid, GEMM_THREADS, SMEM, st>>>(tmA, tmB, tmC, kp);
+  kern<<<grid, GEMM_THREADS, SMEM, st>>>(tmA, tmB, kp);
   PF_CHECK_LAUNCH("gemm_taps_kernel");
   return PF_OK;
 }
 
-// tile width pf_gemm_taps runs with: the caller's request, else the heuristic; the staged (TMA-store) epilogue
-// that carries the fused-LayerNorm statistics has no 256-wide variant
+// tile width pf_gemm_taps runs with: the caller's request, else the heuristic. A statistics PRODUCER always uses the
+// width the heuristic derives from N: the slot partition of the row sums (and so their fp32 rounding) must not depend
+// on a per-call request, or a sharded rank would not reproduce the full batch.
 static int resolve_block_n(const pf_gemm_args* a) {
-  int bn = (a->block_n & 0xffff) ? (a->block_n & 0xffff) : pf_gemm_pick_block_n(a->N, a->act);
-  // a statistics PRODUCER always uses the width the heuristic derives from N: the slot partition of the row sums (and so
-  // their fp32 rounding) must not depend on M-specific tuning, or a sharded rank would not reproduce the full batch
-  if (a->row_stats_out) bn = pf_gemm_pick_block_n(a->N, a->act);
-  if ((a->row_stats_out || a->ln_stats) && a->act != PF_ACT_GEGLU && bn == 256) bn = 128;
-  return bn;
+  return a->block_n && !a->row_stats_out ? a->block_n : pf_gemm_pick_block_n(a->N, a->act);
 }
 
 }  // namespace pf
@@ -672,8 +521,8 @@ extern "C" int pf_gemm_row_stats_slots(const pf_gemm_args* a) {
 }
 
 extern "C" int pf_gemm_pick_block_n(int N, int act) {
-  // GEGLU tiles are epilogue-bound (one erf-GELU per output): the 256-wide tile halves the per-tile fixed cost
-  if (act == PF_ACT_GEGLU && N % 256 == 0) return 256;
+  // GEGLU runs only at the 256-wide tile: its value and gate columns lie 128 apart in one thread's fragment
+  if (act == PF_ACT_GEGLU) return N % 256 == 0 ? 256 : 0;
   if (N % 160 == 0) return 160;
   if (N % 128 == 0) return 128;
   if (N % 64 == 0) return 64;
@@ -722,15 +571,24 @@ extern "C" int pf_gemm_taps(const pf_gemm_args* a, void* stream) {
   PF_CHECK_ARG(!a->residual || a->res_dtype == PF_F32 || a->res_dtype == a->dtype,
                "pf_gemm_taps: res_dtype must be f32 or dtype");
   PF_CHECK_ARG(a->act >= PF_ACT_NONE && a->act <= PF_ACT_QUICK_GELU, "pf_gemm_taps: unknown act %d", a->act);
-  // block_n: low 16 bits = tile width (0 = auto); the high bits are ignored (one schedule)
-  int bn = pf::resolve_block_n(a);
-  PF_CHECK_ARG(bn == 64 || bn == 128 || bn == 160 || bn == 256, "pf_gemm_taps: unsupported block_n %d (N=%d)", bn, a->N);
+  const int bn = pf::resolve_block_n(a);
+  const bool geglu = a->act == PF_ACT_GEGLU;
+  const bool plain16 = a->map_mode == 0 && a->out_dtype == a->dtype && (!a->residual || a->res_dtype == a->dtype);
+  if (geglu) {  // only the persistent linear GEMM has a GEGLU epilogue
+    PF_CHECK_ARG(bn == 256, "pf_gemm_taps: GEGLU runs only at block_n 256, not %d (N=%d)", bn, a->N);
+    PF_CHECK_ARG(a->num_taps == 1, "pf_gemm_taps: GEGLU needs one tap, not %d", a->num_taps);
+    PF_CHECK_ARG(a->map_mode == 0 && a->out_dtype == a->dtype,
+                 "pf_gemm_taps: GEGLU needs map_mode 0 and a 16-bit output");
+    PF_CHECK_ARG(a->k_splits <= 1 && !a->residual && !a->rowbias,
+                 "pf_gemm_taps: GEGLU takes no split-K, residual or rowbias");
+  } else {
+    PF_CHECK_ARG(bn == 64 || bn == 128 || bn == 160, "pf_gemm_taps: unsupported block_n %d (N=%d); 256 only with GEGLU",
+                 bn, a->N);
+  }
   PF_CHECK_ARG(a->N % bn == 0, "pf_gemm_taps: N=%d not a multiple of block_n=%d", a->N, bn);
-  const int n_out = a->act == PF_ACT_GEGLU ? a->N / 2 : a->N;
+  const int n_out = geglu ? a->N / 2 : a->N;
   PF_CHECK_ARG(a->out_ld % 8 == 0 && a->out_ld >= n_out, "pf_gemm_taps: bad out_ld %d", a->out_ld);
   PF_CHECK_ARG(!a->residual || (a->res_ld % 8 == 0 && a->res_ld >= n_out), "pf_gemm_taps: bad res_ld %d", a->res_ld);
-  PF_CHECK_ARG(!(a->act == PF_ACT_GEGLU && (a->residual || a->rowbias)),
-               "pf_gemm_taps: GEGLU epilogue takes no residual/rowbias");
   if (a->map_mode == 1) {
     PF_CHECK_ARG(a->Hm > 0 && a->Wm > 0 && a->Hout > 0 && a->Wout > 0 && a->M % (a->Hm * a->Wm) == 0,
                  "pf_gemm_taps: bad image map Hm=%d Wm=%d M=%d", a->Hm, a->Wm, a->M);
@@ -805,27 +663,25 @@ extern "C" int pf_gemm_taps(const pf_gemm_args* a, void* stream) {
   kp.ln_colsum = a->ln_colsum;
   kp.ln_inv_k = 1.0f / float((long long)a->Kc * a->num_taps);
   kp.ln_eps = a->ln_eps;
-  PF_CHECK_ARG(kp.k_splits == 1 || (a->splitk_ws && a->act != PF_ACT_GEGLU && kp.k_splits <= kp.num_units),
-               "pf_gemm_taps: split-K needs a workspace, no GEGLU and k_splits <= (tap window, channel slab) units");
-  const bool fused_ln = a->row_stats_out || a->ln_stats;
-  if (fused_ln) {
+  PF_CHECK_ARG(kp.k_splits == 1 || (a->splitk_ws && kp.k_splits <= kp.num_units),
+               "pf_gemm_taps: split-K needs a workspace and k_splits <= (tap window, channel slab) units");
+  if (a->row_stats_out || a->ln_stats) {  // fused LayerNorm: only the persistent linear GEMM folds it
     PF_CHECK_ARG(kp.k_splits == 1, "pf_gemm_taps: fused LayerNorm does not combine with split-K");
     PF_CHECK_ARG(!a->ln_stats || (a->ln_colsum && a->ln_slots > 0 && a->ln_slots % 2 == 0 && a->ln_eps > 0.f &&
                                   (reinterpret_cast<uintptr_t>(a->ln_stats) & 15) == 0),
                  "pf_gemm_taps: ln_stats needs ln_colsum, ln_slots and ln_eps");
-    const bool plain16 = a->map_mode == 0 && a->out_dtype == a->dtype && (!a->residual || a->res_dtype == a->dtype);
-    PF_CHECK_ARG(a->act == PF_ACT_GEGLU ? !a->row_stats_out : plain16,
+    PF_CHECK_ARG(a->num_taps == 1 && !a->rowbias, "pf_gemm_taps: fused LayerNorm needs one tap and no rowbias");
+    PF_CHECK_ARG(plain16 && !(geglu && a->row_stats_out),
                  "pf_gemm_taps: fused LayerNorm needs the plain row map with 16-bit output (consumer: or GEGLU)");
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (kp.k_splits > 1) {
-    int rc;
+    int rc = PF_ERR_UNSUPPORTED;
     switch (bn) {
       // few tiles of 90-360 K-slabs, planned at about one CTA per SM: nothing to co-schedule, so the long rings
-      case 64: rc = launch_gemm<64, 8, 1, false>(a, kp, st); break;
-      case 128: rc = launch_gemm<128, 6, 1, false>(a, kp, st); break;
-      case 160: rc = launch_gemm<160, 5, 1, false>(a, kp, st); break;
-      default: rc = launch_gemm<256, 4, 1, false>(a, kp, st); break;
+      case 64: rc = launch_gemm<64, 8, 1>(a, kp, st); break;
+      case 128: rc = launch_gemm<128, 6, 1>(a, kp, st); break;
+      case 160: rc = launch_gemm<160, 5, 1>(a, kp, st); break;
     }
     if (rc) return rc;
     const long long total = (long long)a->M * (a->N / 8);
@@ -835,25 +691,12 @@ extern "C" int pf_gemm_taps(const pf_gemm_args* a, void* stream) {
     return PF_OK;
   }
   // one-tap, plain-row-map calls with 16-bit output and 16-bit (or no) residual and no row bias: the persistent linear
-  // GEMM (gemm_linear.cu). It runs GEGLU at the 256-wide tile and every other epilogue at 64, 128 and 160 wide.
-  const bool plain16 = a->map_mode == 0 && a->out_dtype == a->dtype && (!a->residual || a->res_dtype == a->dtype);
-  if (a->num_taps == 1 && plain16 && !a->rowbias && (a->act == PF_ACT_GEGLU) == (bn == 256))
-    return launch_gemm_linear(a, kp, bn, st);
-  // staged TMA-store epilogue: plain row map, 16-bit output, 16-bit (or no) residual, no GEGLU
-  const bool epi_tma = a->map_mode == 0 && a->out_dtype == a->dtype && a->act != PF_ACT_GEGLU &&
-                       (!a->residual || a->res_dtype == a->dtype) && bn != 256;
-  if (epi_tma) {
-    switch (bn) {
-      case 64: return launch_gemm<64, 4, 2, true>(a, kp, st);
-      case 128: return launch_gemm<128, 3, 2, true>(a, kp, st);
-      case 160: return launch_gemm<160, 3, 2, true>(a, kp, st);
-    }
-  }
+  // GEMM (gemm_linear.cu). The checks above leave every GEGLU and fused-LayerNorm call in this class.
+  if (a->num_taps == 1 && plain16 && !a->rowbias) return launch_gemm_linear(a, kp, bn, st);
   switch (bn) {
-    case 64: return launch_gemm<64, 4, 2, false>(a, kp, st);
-    case 128: return launch_gemm<128, 3, 2, false>(a, kp, st);
-    case 160: return launch_gemm<160, 3, 2, false>(a, kp, st);
-    case 256: return launch_gemm<256, 4, 1, false>(a, kp, st);
+    case 64: return launch_gemm<64, 4, 2>(a, kp, st);
+    case 128: return launch_gemm<128, 3, 2>(a, kp, st);
+    case 160: return launch_gemm<160, 3, 2>(a, kp, st);
   }
   return PF_ERR_UNSUPPORTED;
 }

@@ -29,26 +29,14 @@ def _st():
     return C.c_void_p(_lib.stream_ptr())
 
 
-# optional per-shape tile choice measured by scripts/tune_gemm.py: (M, N, Kc, taps) -> block_n (absent: pf_gemm_pick_block_n)
+# call log: a list while set, one (M, N, Kc, num_taps, act, image_map given, residual given, fp32 out) per gemm_taps
+# call; tests/test_gpu_contracts.py checks that its call table covers what the models log
 GEMM_LOG = None
 # Split-K (pf_gemm_splitk_plan: only skinny deep-K problems — output tiles for at most half the SMs, >= 64 K-slabs, i.e. the 8x8 / 16x16-level
 # convolutions of a small batch, which otherwise stream their weights through a handful of SMs). The K partition depends on the
 # problem's M, so a sharded rank and the single-GPU run round a few convolutions differently (fp32 summation order):
 # PF_SPLIT_K=0 (or ops.SPLIT_K = False) restores the bit-identical sharded == unsharded behaviour the tests check.
 SPLIT_K = __import__("os").environ.get("PF_SPLIT_K", "1") != "0"
-_TUNED: dict = {}
-
-
-def _load_tuning() -> None:
-    import json
-    from pathlib import Path
-    f = Path(__file__).with_name("gemm_tuning.json")
-    if f.exists():
-        for k, v in json.loads(f.read_text()).get("choice", {}).items():
-            _TUNED[tuple(int(x) for x in k.split(","))] = int(v)
-
-
-_load_tuning()
 
 
 def pick_block_n(n: int, act: int = PF_ACT_NONE) -> int:
@@ -79,11 +67,6 @@ def gemm_taps(A: Tensor, B: Tensor, out: Tensor, *, M: int, Kc: int, taps: Seque
     a.M, a.N, a.Kc, a.num_taps = int(M), B.shape[0], int(Kc), len(taps)
     for i, t in enumerate(taps):
         a.tap_off[i] = int(t)
-    if block_n == -1:  # heuristic only (tuner baseline)
-        block_n = 0
-    elif not block_n and act != PF_ACT_GEGLU:
-        block_n = _TUNED.get((int(M), B.shape[0], int(Kc), len(taps), int(image_map is not None),
-                              int(residual is not None)), 0)  # tile width
     a.block_n = int(block_n)
     if GEMM_LOG is not None:
         GEMM_LOG.append((int(M), B.shape[0], int(Kc), len(taps), int(act), image_map is not None,

@@ -64,7 +64,7 @@ def main():
     windows = CI // 64 * 3  # one per kernel row and channel slab
     m_tiles = (M + 127) // 128
     rows = []
-    for bn in (64, 128, 160, 256):
+    for bn in (64, 128, 160):
         fns = [(lambda a=a, o=o: ops.gemm_taps(a, B, o, M=M, Kc=CI, taps=taps, block_n=bn,
                                                image_map=(1, M, 0, 0, 1, M))) for a, o in zip(As, outs)]
         with ClockSampler(dev.index or 0) as clk:

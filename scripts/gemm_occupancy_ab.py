@@ -35,8 +35,9 @@ sys.path.insert(0, str(ROOT))
 T64, T32, T16 = 16 * 64 * 64, 16 * 32 * 32, 16 * 16 * 16  # tokens of the 16 view images at the three UNet levels
 
 # name -> kind, sizes. conv: (images, H, W, Cin, Cout), 3x3 pad 1 over the zero-haloed image, halo-dropping row map
-# (direct stores). lin: (M, K, N) with the plain row map (TMA tile stores); flags: ln = LayerNorm consumer, res =
-# 16-bit residual, stats = row-statistics producer, geglu = GEGLU projection (direct stores, widest tile).
+# (direct stores). lin: (M, K, N) with the plain row map (the persistent linear GEMM, TMA tile stores); flags:
+# ln = LayerNorm consumer, res = 16-bit residual, stats = row-statistics producer, geglu = GEGLU projection
+# (256-wide tile).
 SHAPES = {
     "conv3x3_320_16x64x64": ("conv", (16, 64, 64, 320, 320)),       # the dominant conv of the step, 160-wide
     "conv3x3_640_16x32x32": ("conv", (16, 32, 32, 640, 640)),

@@ -5,11 +5,9 @@
 Builds the model, inputs and sampler as `bench.py --gpus 1` does, runs 4 eager warm-up steps (camera tables, weights,
 allocator), then profiles exactly one eager step with torch.profiler (CUDA activities only) and sums the device time
 of every kernel by family. The tap-GEMM is split into classes by its template arguments
-<BLOCK_N, STAGES, CTAS, BF16, EPI_TMA>:
-  conv (direct store)   EPI_TMA = false, two CTAs per SM: the convolutions (and fp32-output linears)
-  split-K partials      EPI_TMA = false, one CTA per SM, BLOCK_N < 256: the deep-K convolutions of small images
-  linear (TMA store)    EPI_TMA = true: plain-row-map calls the persistent linear GEMM does not take (multi-tap, row bias)
-  GEGLU 256-wide        BLOCK_N = 256
+<BLOCK_N, STAGES, CTAS, BF16>:
+  conv (direct store)   two CTAs per SM: the convolutions (and fp32-output or row-bias GEMMs)
+  split-K partials      one CTA per SM: the deep-K convolutions of small images
 The persistent linear GEMM, gemm_linear_kernel<BLOCK_N, STAGES, GEGLU, BF16>, which runs the one-tap, plain-row-map
 calls with 16-bit output (the linear layers and 1x1 shortcuts), is split by width:
   linear GEMM           the 64-, 128- and 160-wide tiles
@@ -30,7 +28,7 @@ import torch  # noqa: E402
 
 import bench  # noqa: E402
 
-GEMM_RE = re.compile(r"gemm_taps_kernel<(\d+),\s*(\d+),\s*(\d+),\s*(\w+),\s*(\w+)>")
+GEMM_RE = re.compile(r"gemm_taps_kernel<(\d+),\s*(\d+),\s*(\d+),\s*(\w+)>")
 LINEAR_RE = re.compile(r"gemm_linear_kernel<(\d+),\s*(\d+),\s*(\w+),\s*(\w+)>")
 
 
@@ -40,12 +38,7 @@ def family(name: str) -> str:
         return "linear GEMM GEGLU 256-wide" if m.group(3) == "true" else "linear GEMM 64/128/160-wide"
     m = GEMM_RE.search(name)
     if m:
-        bn, _, ctas, _, epi_tma = m.groups()
-        if int(bn) == 256:
-            return "tap-GEMM GEGLU 256-wide"
-        if epi_tma == "true":
-            return "tap-GEMM linear (TMA store)"
-        return "tap-GEMM conv (direct store)" if int(ctas) == 2 else "tap-GEMM split-K partials"
+        return "tap-GEMM conv (direct store)" if int(m.group(3)) == 2 else "tap-GEMM split-K partials"
     base = name.split("(")[0]
     base = re.sub(r"^void\s+", "", base)
     base = re.sub(r"<.*", "", base)

@@ -41,6 +41,19 @@ def test_bad_arguments_fail_loudly_without_gpu():
     assert lib.pf_gemm_pick_block_n(100, 0) == 0
 
 
+def _gemm_args(**fields):
+    """A valid one-tap fp16 pf_gemm_args (M = 512, N = Kc = 320) with `fields` overridden; its pointers are never
+    dereferenced."""
+    from panfusion_b200 import _lib
+    a = _lib.GemmArgs()
+    a.A, a.a_rows, a.a_ld, a.B, a.b_ld, a.dtype = 0x10000, 512, 320, 0x20000, 320, 1
+    a.M, a.N, a.Kc, a.num_taps = 512, 320, 320, 1
+    a.out, a.out_ld, a.out_dtype = 0x30000, 320, 1
+    for k, v in fields.items():
+        setattr(a, k, v)
+    return a
+
+
 @pytest.mark.parametrize("field,value,extra,operand", [
     ("residual", 0x40008, dict(res_ld=320, res_dtype=1), b"residual"),
     ("rowbias", 0x40004, dict(rowbias_ld=320, rows_per_group=64), b"rowbias"),
@@ -55,15 +68,35 @@ def test_misaligned_epilogue_operands_are_rejected_without_gpu(field, value, ext
     import ctypes as C
     from panfusion_b200 import _lib
     lib = _lib.lib()
-    a = _lib.GemmArgs()
-    a.A, a.a_rows, a.a_ld, a.B, a.b_ld, a.dtype = 0x10000, 512, 320, 0x20000, 320, 1
-    a.M, a.N, a.Kc, a.num_taps = 512, 320, 320, 1
-    a.out, a.out_ld, a.out_dtype = 0x30000, 320, 1
-    setattr(a, field, value)
-    for k, v in extra.items():
-        setattr(a, k, v)
+    a = _gemm_args(**{field: value}, **extra)
     rc = lib.pf_gemm_taps(C.byref(a), None)
     assert rc == -1 and operand in lib.pf_last_error(), lib.pf_last_error()
+
+
+_GEGLU = dict(act=3, N=512, out_ld=256)  # PF_ACT_GEGLU: 512 packed columns -> 256 outputs
+_LN = dict(ln_stats=0x40000, ln_slots=4, ln_colsum=0x50000, ln_eps=1e-5)
+
+
+@pytest.mark.parametrize("fields,cause", [
+    (dict(_GEGLU, block_n=128), b"GEGLU runs only at block_n 256"),
+    (dict(_GEGLU, N=640, out_ld=320, block_n=160), b"GEGLU runs only at block_n 256"),
+    (dict(_GEGLU, out_dtype=0), b"GEGLU needs map_mode 0 and a 16-bit output"),
+    (dict(_GEGLU, num_taps=2, b_ld=640), b"GEGLU needs one tap"),
+    (dict(row_stats_out=0x40000, num_taps=2, b_ld=640), b"fused LayerNorm needs one tap and no rowbias"),
+    (dict(_LN, rowbias=0x60000, rowbias_ld=320, rows_per_group=64), b"fused LayerNorm needs one tap and no rowbias"),
+    (dict(N=512, block_n=256), b"unsupported block_n 256"),
+    (dict(block_n=64 | (1 << 16)), b"unsupported block_n 65600"),
+], ids=["geglu_bn128", "geglu_bn160", "geglu_fp32_out", "geglu_two_taps", "row_stats_two_taps", "ln_stats_rowbias",
+        "bn256_without_geglu", "bn_high_bits"])
+def test_gemm_contract_is_checked_without_gpu(fields, cause):
+    """GEGLU runs only at block_n = 256 with one tap and a 16-bit output, the fused LayerNorm needs one tap and no row
+    bias, and block_n is 0, 64, 128, 160 or (GEGLU) 256: pf_gemm_taps refuses anything else before any CUDA call, with
+    a message that names the cause."""
+    import ctypes as C
+    from panfusion_b200 import _lib
+    lib = _lib.lib()
+    rc = lib.pf_gemm_taps(C.byref(_gemm_args(**fields)), None)
+    assert rc == -1 and cause in lib.pf_last_error(), lib.pf_last_error()
 
 
 def test_no_cpu_path():
@@ -121,14 +154,14 @@ def test_camera_table_dedup():
 
 
 def test_row_stats_slots_ignore_tile_requests():
-    """A fused-LayerNorm PRODUCER's slot layout is a function of N alone (never of a tile-width request or of tuning), and the
-    query gives the same answer before and after the caller has filled in row_stats_out."""
+    """A fused-LayerNorm PRODUCER's slot layout is a function of N alone (never of a tile-width request), and the query
+    gives the same answer before and after the caller has filled in row_stats_out."""
     import ctypes as C
     from panfusion_b200 import _lib
     lib = _lib.lib()
     for n, want in ((320, 4), (640, 8), (1280, 16), (128, 2), (64, 2)):
         seen = set()
-        for req in (0, 64, 128, 64 | (2 << 16), 256 | (1 << 16)):
+        for req in (0, 64, 128, 160, 256):
             a = _lib.GemmArgs()
             a.N, a.M, a.Kc, a.num_taps, a.block_n = n, 512, n, 1, req
             seen.add(lib.pf_gemm_row_stats_slots(C.byref(a)))

@@ -55,7 +55,7 @@ def _gemm(checks, name, A, B, out, launches=1, **kw):
     if "ln" in kw:
         ref_kw["ln_eps"] = kw["ln"][2]
     if kw.get("act") == ops.PF_ACT_GEGLU:
-        ref_kw["geglu_bn"] = kw["block_n"] & 0xffff
+        ref_kw["geglu_bn"] = kw["block_n"]
     ref, bound = ct.tap_gemm_ref(A, B, out.shape[0], out.dtype, **ref_kw)
     l0 = ops.LAUNCHES
     r = ops.gemm_taps(A, B, out, **kw)
@@ -90,7 +90,8 @@ def case_temb_mlp(g, dev, dt):
 
 def case_linear_edge_m(g, dev, dt):
     """map_mode 0 at M = 1, 127, 129 (a partial first / last tile), one tile width each: fp32 out + GELU (64),
-    16-bit residual + SiLU through the TMA-store epilogue (128), per-group row bias (160)."""
+    16-bit residual + SiLU through the persistent linear GEMM (128), per-group row bias through the tap-GEMM's direct
+    stores (160)."""
     from panfusion_b200 import ops
     checks = []
     A = _rand(g, (129, 640), dev, dt)

@@ -3,7 +3,7 @@
 Taps whose offsets lie within 8 rows of each other share one A window of 136 rows, and each tap's wgmma operand starts
 1..8 rows into it. These cases put taps at every shift inside a window, windows that start before row 0 and end past
 a_rows (zero-filled by the TMA), groups of 1, 2, 3 and 9 taps in one call, taps passed out of offset order, and spans
-exactly at the limit and one past it, at every tile width, with the direct-store, TMA-store and split-K epilogues.
+exactly at the limit and one past it, at every tile width, with fp32 and 16-bit direct stores and split-K.
 M = 1000 is not a multiple of 128, so the first and the last, partial, M-tile both read clipped windows."""
 import pytest
 import torch
@@ -63,7 +63,7 @@ def test_tap_windows_direct_store(cuda_device, taps, block_n, dtype):
 @pytest.mark.parametrize("dtype", DTYPES, ids=["f16", "bf16"])
 @pytest.mark.parametrize("taps", list(TAP_SETS), ids=list(TAP_SETS))
 def test_tap_windows_tma_store(cuda_device, taps, dtype):
-    """16-bit output with a 16-bit residual: the TMA-store epilogue."""
+    """16-bit output with a 16-bit residual: the direct-store epilogue's 16-bit path."""
     from panfusion_b200 import ops
     tp = TAP_SETS[taps]
     A, B, bias = _operands(tp, dtype, cuda_device, seed=1)
