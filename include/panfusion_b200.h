@@ -488,6 +488,41 @@ int pf_clip_score(const float* img_emb, const float* txt_emb, int B, int D, floa
                   void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * HorizonNet layout network (models/horizonnet/HorizonNet.py `net` = external/HorizonNet/model.py
+ * HorizonNet('resnet50', use_rnn=True)). Activations are channels-last fp16 [B, H, W, C]; wrap_lr_pad's LR_PAD(p) +
+ * Conv2d(padding=(p, 0)) (rows zero-padded, columns wrapped, corners zero) is addressing inside pf_hnet_conv. The LSTM's
+ * input projections are pf_gemm_taps calls; the rows of the LSTM input and output are (t, b) ordered: row t * B + b.
+ * pf_hnet_prep (_prepare_x): src fp32 [B, C, 512, 1024] (C >= 3, channels 0..2 read) -> dst fp16 [B, 512, 1024, 16] =
+ *   (x - mean) / std as two fp32 ops with ImageNet mean / std, rounded once; channels 3..15 are zero. */
+int pf_hnet_prep(const float* src, int B, int C, int H, int W, void* dst, void* stream);
+/* Conv2d with BN folded into w / bias (fp64 on the host, the conv bias included), k x k with padding k / 2: rows
+ * zero-padded, columns wrapped (a no-op for k = 1), stride (stride_h, stride_w) in {(1, 1), (2, 2), (2, 1)}; then
+ * v = acc + bias (+ residual if non-NULL), ReLU if relu != 0: the residual is added BEFORE the ReLU (torchvision's
+ * Bottleneck). x fp16 [B, H, W, Cin], w fp16 [k*k][Cin][Cout] (tap-major ky, kx), bias fp32 [Cout], residual fp16
+ * [B, Ho, Wo, Cout] or NULL, out [B, Ho, Wo, Cout] fp16 or fp32 (out_dtype). k in {1, 3, 7}; Cin 16 (the stem, Cout 64)
+ * or a multiple of 64; Cout 32, 64 or a multiple of 128. Anything else is PF_ERR_INVALID. */
+int pf_hnet_conv(const void* x, int B, int H, int W, int Cin, const void* w, const float* bias, int Cout, int k,
+                 int stride_h, int stride_w, int relu, const void* residual, void* out, int out_dtype, void* stream);
+/* GlobalHeightConv's tail for one scale: x fp16 [B, h, w, C] -> cat(x[..., -1:], x, x[..., :1]), bilinear
+ * (align_corners=False) to width f * (w + 2), f = T / w, height unchanged, [..., f:-f], reshape(B, C * h, T) — written
+ * as out fp16 [T * B, 1024] row t * B + b, columns [out_off + c * h + y]. Exact fp32 weights, torch's expression; T % w
+ * == 0 and out_off + C * h <= 1024. */
+int pf_hnet_height_upsample(const void* x, int B, int h, int w, int C, int T, void* out, int out_off, void* stream);
+/* Recurrence of one bidirectional nn.LSTM(1024 -> 512) layer with zero h0 / c0, both directions in one launch:
+ *   gates = xproj[t] + W_hh h_{t-1}; c = sigmoid(f) c + sigmoid(i) tanh(g); h = sigmoid(o) tanh(c)   (fp32, i f g o)
+ * the reverse direction runs t = T-1 -> 0. xproj fp32 [T * B, 4096] = x W_ih^T + b_ih + b_hh of [fwd | bwd]; whh fp16
+ * [2][16][128][512]: direction, CTA r, its rows (gate q, unit u) = W_hh[q * 512 + 32 r + u] (16-byte aligned). out fp16
+ * [T * B, 1024] = [h_fwd | h_bwd]. 1 <= B <= 16; each sample's arithmetic is the same for any B. One 16-CTA thread-block
+ * cluster per direction, W_hh in shared memory for all steps, h exchanged through distributed shared memory. A device
+ * that cannot hold such a cluster gives PF_ERR_UNSUPPORTED without launching. */
+int pf_lstm_bidir(const float* xproj, const void* whh, int T, int B, void* out, void* stream);
+/* clusters <- cudaOccupancyMaxActiveClusters of pf_lstm_bidir's 16-CTA clusters on the current device */
+int pf_lstm_bidir_clusters(int* clusters);
+/* Linear(1024, 12) in fp32 over x fp16 [T * B, 1024] (every output summed in a fixed order), then view(T, B, 3, 4)
+ * .permute(1, 2, 0, 3): cor fp32 [B, 1, 4T] (channel 0), bon fp32 [B, 2, 4T] (channels 1, 2). w fp32 [12, 1024]. */
+int pf_hnet_head(const void* x, int T, int B, const float* w, const float* bias, float* bon, float* cor, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * View-sharded step (SURVEY.md 8e): device-initiated all-gather over NVLink peer mappings, capturable in a CUDA graph.
  * The reference has no model parallelism (Lightning DDP over prompts, main.py:63); this is the exchange the view partition
  * needs: models/pano/modules.py:44-48 lets every panorama query attend to the keys / values of ALL views, so each rank

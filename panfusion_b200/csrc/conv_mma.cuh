@@ -12,6 +12,9 @@
 // a template parameter so that neither kind of layer pays for the other's address test in the load loop.
 // The epilogue adds the bias (BN folded), applies ReLU, adds an optional fp16 residual [M][Cout] and stores fp16 or fp32
 // at out[m * out_ld + out_off + col] for col < Cout, so a branch writes straight into its slice of a concat buffer.
+// Two more template parameters serve HorizonNet's ResNet-50 (horizonnet.cu) without costing the other layers anything:
+// RES_BEFORE_RELU adds the residual before the ReLU (torchvision's Bottleneck, relu(bn3(conv3) + identity)), and
+// STRIDE_HW takes the column stride from stride_w instead of stride (ConvCompressH's stride (2, 1)).
 #pragma once
 #include "pf_common.cuh"
 
@@ -35,6 +38,7 @@ struct ConvArgs {
   int Cw;              // packed weight / bias width (Cout rounded up to the N tile)
   int out_ld, out_off;  // output row stride and channel offset, in elements
   int M;
+  int stride_w;  // column stride, read only by STRIDE_HW instances
 };
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {
@@ -70,7 +74,7 @@ struct ConvTile {
   static constexpr int NT = BN / 16;                    // n8 tiles per warp
 };
 
-template <int KC, int BN, bool CIRC>
+template <int KC, int BN, bool CIRC, bool RES_BEFORE_RELU = false, bool STRIDE_HW = false>
 __global__ void __launch_bounds__(kThreads)
 conv_mma_kernel(ConvArgs a) {
   using T = ConvTile<KC, BN>;
@@ -93,7 +97,7 @@ conv_mma_kernel(ConvArgs a) {
       const int b = m / HoWo, r = m % HoWo;
       a_base[i] = b * a.H;
       a_y[i] = (r / a.Wo) * a.stride - a.ph;
-      a_x[i] = (r % a.Wo) * a.stride - a.pw;
+      a_x[i] = (r % a.Wo) * (STRIDE_HW ? a.stride_w : a.stride) - a.pw;
     } else {
       a_base[i] = 0;
       a_y[i] = -(1 << 20);  // never inside the image: zero-filled
@@ -184,11 +188,16 @@ conv_mma_kernel(ConvArgs a) {
         const int m = m0 + wm * 32 + mt * 16 + (lane >> 2) + h * 8;
         if (m >= a.M) continue;
         float v0 = acc[mt][nt][2 * h] + bias0, v1 = acc[mt][nt][2 * h + 1] + bias1;
+        if (RES_BEFORE_RELU && a.residual) {
+          const float2 r = __half22float2(*reinterpret_cast<const __half2*>(a.residual + (size_t)m * a.Cout + col));
+          v0 += r.x;
+          v1 += r.y;
+        }
         if (a.relu) {
           v0 = fmaxf(v0, 0.f);
           v1 = fmaxf(v1, 0.f);
         }
-        if (a.residual) {
+        if (!RES_BEFORE_RELU && a.residual) {
           const float2 r = __half22float2(*reinterpret_cast<const __half2*>(a.residual + (size_t)m * a.Cout + col));
           v0 += r.x;
           v1 += r.y;
@@ -202,19 +211,20 @@ conv_mma_kernel(ConvArgs a) {
     }
 }
 
-template <int KC, int BN, bool CIRC>
+template <int KC, int BN, bool CIRC, bool RES_BEFORE_RELU = false, bool STRIDE_HW = false>
 int launch_conv(const ConvArgs& a, cudaStream_t st) {
   using T = ConvTile<KC, BN>;
   static bool attr_set = false;  // per-kernel opt-in to > 48 KB of dynamic shared memory
   if (!attr_set) {
     const int rc = check_cuda(
-        cudaFuncSetAttribute(conv_mma_kernel<KC, BN, CIRC>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SMEM),
+        cudaFuncSetAttribute(conv_mma_kernel<KC, BN, CIRC, RES_BEFORE_RELU, STRIDE_HW>,
+                             cudaFuncAttributeMaxDynamicSharedMemorySize, T::SMEM),
         "cudaFuncSetAttribute(conv_mma_kernel)");
     if (rc) return rc;
     attr_set = true;
   }
   const dim3 grid((unsigned)((a.M + kBM - 1) / kBM), (unsigned)(a.Cw / BN));
-  conv_mma_kernel<KC, BN, CIRC><<<grid, kThreads, T::SMEM, st>>>(a);
+  conv_mma_kernel<KC, BN, CIRC, RES_BEFORE_RELU, STRIDE_HW><<<grid, kThreads, T::SMEM, st>>>(a);
   PF_CHECK_LAUNCH("conv_mma_kernel");
   return PF_OK;
 }
