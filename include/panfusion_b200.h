@@ -420,6 +420,72 @@ int pf_frechet_fp64(const double* sum1, const double* cov_sum1, long long n1, co
                     const double* cov_sum2, long long n2, int d, double* ws, double* out, int* sweeps, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * FAED autoencoder training (models/faed/FAED.py:13-33, AutoEncoder of models/faed/modules.py). Activations are
+ * channels-last fp16 [B, H, W, C]. Activation gradients carry the loss scale S = scale[0] (device double, a power of
+ * two): the seed is sign * S, and every fp32 parameter gradient is reduced as sum * (inv_n / S) with inv_n = 1 / N of the
+ * L1 mean. Each reduction sums fixed-size chunks (sizes depend on the shape only) in a fixed order: no float atomics,
+ * the bits do not depend on the grid. flag: device int set to 1 by any non-finite loss or parameter gradient.
+ * pf_faedt_prep: pano fp32 [B, 3, H, W] -> dst fp16 [B, H, W, 16], channels 3..15 zero. */
+int pf_faedt_prep(const float* src, int B, int H, int W, void* dst, void* stream);
+/* Circular convolution on the pf_conv_circ core with bias, no ReLU: rows of x outside [0, H) read zero, columns wrap
+ * (iy = oy*stride + ky - ph, ix = ox*stride + kx - pw mod W). x fp16 [B, H, W, Cin], w fp16 [kh*kw][Cin][Cw] (zero
+ * columns past Cout), bias fp32 [Cw], residual fp16 [B, Ho, Wo, Cout] or NULL (then out_ld == Cout), out fp16 / fp32
+ * (out_dtype) [B, Ho, Wo, out_ld], channels < Cout written. Ho, Wo are given, so the 2x2 phase kernels of a stride-2
+ * adjoint run here too. (Cin, Cw): (16, 32), (32, 32), (32, 64), (>= 64, 32 / 64 / 128) with Cin % 64 == 0 past 64;
+ * anything else is PF_ERR_UNSUPPORTED. Cout even. */
+int pf_faedt_conv(const void* x, int B, int H, int W, int Cin, const void* w, const float* bias, int Cout, int Cw,
+                  int kh, int kw, int stride, int ph, int pw, int Ho, int Wo, const void* residual, void* out,
+                  int out_ld, int out_dtype, void* stream);
+/* Weight and bias gradient of the circular convolution (k, stride, pad as in the forward):
+ * dw [Cout][Cin_w][k][k] (torch layout) = f * sum_p x[p (+) tap, ci] dy[p, co], db [Cout] = f * sum_p dy[p, co] (db may be
+ * NULL), f = inv_n / scale[0]. x fp16 [B, H, W, Cin] (Cin % 8 == 0, <= 128; channels >= Cin_w ignored), dy fp16
+ * [B, Ho, Wo, Cdy] (Cdy % 8 == 0, <= 128; channels >= Cout ignored). ws: pf_faedt_wgrad_ws_floats(...) floats of fp32
+ * per-chunk partials. Tensor-core split-K over pixel chunks, reduced in chunk order. */
+long long pf_faedt_wgrad_ws_floats(int B, int Ho, int Wo, int Cin, int Cdy, int k);
+int pf_faedt_wgrad(const void* x, int B, int H, int W, int Cin, const void* dy, int Ho, int Wo, int Cdy, int Cin_w,
+                   int Cout, int k, int stride, int pad, float* ws, const double* scale, double inv_n, float* dw,
+                   float* db, int* flag, void* stream);
+/* BatchNorm2d in training mode (eps 1e-5) over z fp16 [P, C] (C 32/64/128, P > 1). ws: pf_faedt_bn_ws_floats(P, C).
+ * pf_faedt_bn_stats: per-chunk Welford (count, mean, M2) merged in chunk order (Chan) -> stats fp32 [3][C] = batch
+ * mean, 1 / sqrt(biased var + eps), unbiased var; pending fp32 [2][C] <- (mean, unbiased var), which pf_faedt_adam folds
+ * into the running statistics (momentum 0.1) only if the step is not skipped.
+ * pf_faedt_bn_apply: out = relu?((z - mean) * invstd * gamma + beta) + residual? (fp16 [P, C]).
+ * pf_faedt_bn_bwd: g' = g * (mask > 0) (mask = the ReLU output, or NULL), dz = gamma * invstd * (g' - mean g' -
+ * xhat mean(g' xhat)) fp16; dgamma = f * sum g' xhat, dbeta = f * sum g' (fp32 [C], f = inv_n / scale[0]). */
+long long pf_faedt_bn_ws_floats(long long P, int C);
+int pf_faedt_bn_stats(const void* z, long long P, int C, float* ws, float* stats, float* pending, void* stream);
+int pf_faedt_bn_apply(const void* z, long long P, int C, const float* stats, const float* gamma, const float* beta,
+                      int relu, const void* residual, void* out, void* stream);
+int pf_faedt_bn_bwd(const void* g, const void* mask, const void* z, long long P, int C, const float* stats,
+                    const float* gamma, float* ws, const double* scale, double inv_n, float* dgamma, float* dbeta,
+                    int* flag, void* dz, void* stream);
+/* F.interpolate(scale_factor=2, mode='bilinear', align_corners=False): x fp16 [B, H, W, C] -> out [B, 2H, 2W, C]; the
+ * backward g [B, 2H, 2W, C] -> dx [B, H, W, C] gathers the <= 4x4 outputs each input feeds (no scatter-add). */
+int pf_faedt_upsample(const void* x, int B, int H, int W, int C, void* out, void* stream);
+int pf_faedt_upsample_bwd(const void* g, int B, int H, int W, int C, void* dx, void* stream);
+/* o fp32 [B, H, W, 4] (outconv, channel 3 ignored), target fp32 [B, 3, H, W] or NULL (zeros): pred = tanh(o) (also stored to pred
+ * [B, 3, H, W] unless NULL), loss[0] = mean |pred - target| (fixed-order fp32 sum), seed fp16 [B, H, W, 16] =
+ * sign(pred - target) * (1 - pred^2) * S (sign(0) = 0; channels 3..15 zero). ws: pf_faedt_loss_ws_floats() floats. */
+long long pf_faedt_loss_ws_floats(void);
+int pf_faedt_loss(const float* o, const float* target, int B, int H, int W, const double* scale, float* ws, float* loss,
+                  float* pred, void* seed, int* flag, void* stream);
+/* torch.optim.Adam (foreach=False, no weight decay) over n fp32 params / grads / moments, lr = ctl[0] (device double),
+ * step = ictl[0] + 1; the first n_running floats of `running` become 0.9 running + 0.1 pending. If the flag ictl[3] is
+ * set nothing changes, ctl[1] (the loss scale) halves, the growth tracker ictl[1] resets and ictl[2] (skipped steps)
+ * counts up; otherwise ictl[0] and *num_batches count up and the scale doubles after 2000 clean steps. ictl[3] is
+ * cleared. */
+int pf_faedt_adam(float* params, const float* grads, float* m, float* v, long long n, float* running,
+                  const float* pending, long long n_running, double* ctl, int* ictl, long long* num_batches,
+                  double beta1, double beta2, double eps, void* stream);
+/* w fp32 [Cout][Cin][k][k] -> fwd fp16 [k*k][cin_pad][cw] and, unless dg is NULL, the adjoint's weights: stride 1
+ * (k odd) the flipped kernel [k*k][dg_rows][dg_cw] (dg_rows >= Cout, dg_cw >= Cin); stride 2 (k = 4) the four 2x2 phase
+ * kernels [4 phases (r, c)][4 taps (ty, tx)][dg_rows][dg_cw] = w[.., 3 - 2 ty - r, 3 - 2 tx - c]. */
+int pf_faedt_pack(const float* w, int Cout, int Cin, int k, int stride, void* fwd, int cin_pad, int cw, void* dg,
+                  int dg_rows, int dg_cw, void* stream);
+/* phases fp16 [4][B, H/2, W/2, C] -> dx [B, H, W, C] with dx[b, 2q + r, 2p + c] = phases[2r + c][b, q, p]. */
+int pf_faedt_interleave(const void* phases, int B, int H, int W, int C, void* dx, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * FID and Inception Score (models/pano/EvalPanoGen.py:30-49: torchmetrics FrechetInceptionDistance / InceptionScore over
  * torch-fidelity's FeatureExtractorInceptionV3, the network of torchmetrics' NoTrainInceptionV3). Activations are
  * channels-last fp16 [B, H, W, C]. FID's statistics and distance are pf_faed_stats and pf_frechet_fp64 at d = 2048.

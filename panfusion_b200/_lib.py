@@ -90,6 +90,9 @@ EXPORTS = [
     "pf_allgather_views", "pf_enable_peer_access", "pf_comm_alloc", "pf_comm_free", "pf_ipc_export", "pf_ipc_open",
     "pf_ipc_close", "pf_embed_tokens", "pf_add_noise", "pf_mse_loss_ws_floats", "pf_mse_loss", "pf_gaussian_sample",
     "pf_faed_prep", "pf_conv_circ", "pf_faed_pool", "pf_faed_stats", "pf_frechet_ws_doubles", "pf_frechet_fp64",
+    "pf_faedt_prep", "pf_faedt_conv", "pf_faedt_wgrad_ws_floats", "pf_faedt_wgrad", "pf_faedt_bn_ws_floats",
+    "pf_faedt_bn_stats", "pf_faedt_bn_apply", "pf_faedt_bn_bwd", "pf_faedt_upsample", "pf_faedt_upsample_bwd",
+    "pf_faedt_loss_ws_floats", "pf_faedt_loss", "pf_faedt_adam", "pf_faedt_pack", "pf_faedt_interleave",
     "pf_inception_prep", "pf_conv2d_packed_cout", "pf_conv2d_nhwc", "pf_pool2d_nhwc", "pf_inception_head",
     "pf_inception_score_ws_doubles", "pf_inception_score",
     "pf_clip_prep_taps_ints", "pf_clip_prep_taps", "pf_clip_prep", "pf_clip_embed", "pf_clip_score",
