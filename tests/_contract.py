@@ -1,5 +1,6 @@
-"""fp64 restatements of the tap-GEMM (pf_gemm_taps) and flash-attention (pf_fmha_fwd) contracts of
-include/panfusion_b200.h, and the error bound a correct kernel meets on every output element.
+"""fp64 restatements of the tap-GEMM (pf_gemm_taps), flash-attention (pf_fmha_fwd) and implicit-GEMM convolution
+(pf_conv_circ, pf_faedt_conv, pf_conv2d_nhwc, pf_hnet_conv) contracts of include/panfusion_b200.h, and the error bound
+a correct kernel meets on every output element.
 
 The bound scales with the magnitude of the terms that make up each element, not with max|ref|: an element that is
 small because its terms cancel may carry the rounding of its large terms, but one wrong tap, row or column changes an
@@ -12,6 +13,11 @@ element by about its own magnitude, far above the bound.
              does not round LN(x) to 16 bits, the stand-alone pair does).
   attention  |got - ref| <= 2u * (P @ |V|) + u * |ref| + 2^-20, u = 2^-11 (fp16) / 2^-8 (bf16): the kernel rounds
              P to 16 bits before P V and rounds the output once.
+  conv_mma   |got - ref| <= 2^-14 * (|x| * |w| + |bias| + |residual|) + ulp_out(ref)  (the implicit-GEMM convolution
+             of csrc/conv_mma.cuh behind pf_conv_circ, pf_faedt_conv, pf_conv2d_nhwc and pf_hnet_conv; * is the
+             convolution with the layer's own padding). ReLU is 1-Lipschitz and needs no factor. The deepest K any model
+             passes is HorizonNet's first ConvCompressH, 9 * 2048 = 18432: sqrt(K) * 2^-24 = 8.1e-6, and ten times that
+             rounds to the same power of two, 2^-14 (7.5x there, 9.5x at the tap-GEMM's 9 * 1280).
 
 Every function here runs on whichever device its inputs live on (the CPU tests use the same code at small sizes).
 """
@@ -119,6 +125,64 @@ def merge(parts):
         ref = torch.where(torch.isnan(ref), r, ref)
         bound = torch.where(torch.isnan(bound), b, bound)
     return ref, bound
+
+
+def conv_ref(x, w, bias, *, Cout: int, kh: int, kw: int, stride_h: int, stride_w: int, ph: int, pw: int, circ: bool,
+             relu: bool, out_dtype: torch.dtype, residual=None, res_before_relu: bool = False, Ho: int | None = None,
+             Wo: int | None = None, out_rows: int | None = None, out_ld: int | None = None, out_off: int = 0,
+             chunk: int = 0):
+    """(ref, bound) of one conv_mma launch, both fp64 [out_rows, out_ld] (out_rows >= M = B * Ho * Wo); every element
+    the launch must not write (rows past M, columns outside [out_off, out_off + Cout)) is NaN in both.
+
+    x: the channels-last fp16 input [B, H, W, Cin_pad] (padded channels included); w: the packed fp16 weight
+    [kh * kw][Cin_pad][Cw] (tap-major ky, kx; columns past Cout are ignored); bias: fp32 [>= Cout]; residual: fp16
+    [M, Cout] rows (the kernel reads it with row stride Cout). Input row iy = oy * stride_h + ky - ph reads zero outside
+    [0, H); input column ix = ox * stride_w + kx - pw reads zero outside [0, W), or x[..., ix mod W] when circ (corners
+    zero). Ho / Wo default to the symmetric-padding output size; the stride-2 data-gradient phases pass their own.
+    Epilogue: + bias, then ReLU, then + residual; with res_before_relu the residual goes before the ReLU.
+    `chunk` > 0 computes that many images at a time (full-resolution layers on the device)."""
+    B, H, W, cin = x.shape
+    taps, cin_w, _cw = w.shape
+    assert taps == kh * kw and cin_w == cin, (tuple(x.shape), tuple(w.shape), kh, kw)
+    Ho = (H + 2 * ph - kh) // stride_h + 1 if Ho is None else Ho
+    Wo = (W + 2 * pw - kw) // stride_w + 1 if Wo is None else Wo
+    M = B * Ho * Wo
+    out_rows = M if out_rows is None else out_rows
+    out_ld = Cout if out_ld is None else out_ld
+    dev = x.device
+    wt = w.double().reshape(kh, kw, cin, -1).permute(3, 2, 0, 1)[:Cout].contiguous()
+    wa = wt.abs()
+    rows_end, cols_end = (Ho - 1) * stride_h + kh - ph, (Wo - 1) * stride_w + kw - pw  # exclusive, in input coordinates
+    accs, mags = [], []
+    for b0 in range(0, B, chunk or B):
+        xb = x[b0:b0 + (chunk or B)].double().permute(0, 3, 1, 2)
+        if circ:
+            xb = xb[..., torch.arange(-pw, cols_end, device=dev) % W]
+        else:
+            xb = torch.nn.functional.pad(xb, (pw, max(0, cols_end - W)))
+        xb = torch.nn.functional.pad(xb, (0, 0, ph, max(0, rows_end - H)))
+        conv = lambda a, f: torch.nn.functional.conv2d(a, f, stride=(stride_h, stride_w))[:, :, :Ho, :Wo]
+        accs.append(conv(xb, wt).permute(0, 2, 3, 1).reshape(-1, Cout))
+        mags.append(conv(xb.abs(), wa).permute(0, 2, 3, 1).reshape(-1, Cout))
+        del xb
+    acc, mag = torch.cat(accs), torch.cat(mags)
+    bias64 = bias[:Cout].double().to(dev)
+    acc += bias64
+    err = GEMM_REL * (mag + bias64.abs())
+    res = None if residual is None else residual.reshape(M, Cout).double()
+    if res is not None:
+        err += GEMM_REL * res.abs()
+        if res_before_relu:
+            acc += res
+    if relu:
+        acc = acc.clamp_min(0.0)
+    if res is not None and not res_before_relu:
+        acc += res
+    ref = torch.full((out_rows, out_ld), float("nan"), dtype=torch.float64, device=dev)
+    bound = torch.full_like(ref, float("nan"))
+    ref[:M, out_off:out_off + Cout] = acc
+    bound[:M, out_off:out_off + Cout] = err
+    return ref, bound + ulp_out(ref, out_dtype)
 
 
 def fmha_ref(q, k, v, *, heads: int, head_dim: int, scale: float, bias=None, chunk: int = 1024):

@@ -3,7 +3,10 @@
 Each case computes the exact fp64 result of a small tap-GEMM or attention, rounds it to the output type as a correct
 kernel would, and checks that it passes the bound; then it emulates one subtle kernel bug (a dropped tap, a shifted
 row-bias group, a halo row in the output, a residual read one row off, swapped GEGLU halves, an unmasked ragged key, a
-bias read from the wrong batch) and checks that the bound catches it on at least one element."""
+bias read from the wrong batch) and checks that the bound catches it on at least one element. The convolution cases
+(conv_ref, the contract of csrc/conv_mma.cuh) first pin conv_ref to F.conv2d, then emulate a seam column wrapped to
+zero, a neighbouring column's bias, a dropped K chunk, the residual on the wrong side of the ReLU, a tile row reading the
+previous image, a store past Cout and a shifted output slice."""
 import pytest
 import torch
 
@@ -129,3 +132,159 @@ def test_rows_outside_the_contract_must_stay_untouched():
     with pytest.raises(AssertionError):
         ct.worst_ratio(torch.tensor([[1.0], [0.0]]), ref, bound)
     assert ct.worst_ratio(torch.tensor([[float("nan")], [float("nan")]]), ref, bound) == float("inf")
+
+
+# ---- implicit-GEMM convolution (conv_mma.cuh) -----------------------------------------------------------------------
+
+def _conv_operands(seed, B=2, H=5, W=6, cin=32, cin_pad=32, cout=6, cw=32, k=3, res=False, offset=0.0):
+    """fp16 channels-last input (channels past cin zero), the packed fp16 weight [k*k][cin_pad][cw] (zero past cin and
+    cout), an fp32 bias over cw columns and an optional fp16 residual for the stride-1 'same' output."""
+    g = torch.Generator().manual_seed(seed)
+    x = torch.zeros(B, H, W, cin_pad)
+    x[..., :cin] = torch.randn(B, H, W, cin, generator=g) + offset
+    w = torch.randn(cout, cin, k, k, generator=g, dtype=torch.float64) / (cin * k * k) ** 0.5
+    wp = torch.zeros(k * k, cin_pad, cw, dtype=torch.float64)
+    wp[:, :cin, :cout] = w.permute(2, 3, 1, 0).reshape(k * k, cin, cout)
+    bias = torch.randn(cw, generator=g) * 0.5
+    r = torch.randn(B * H * W, cout, generator=g).half() if res else None
+    return x.half(), wp.half(), bias, r
+
+
+def _conv_kw(cout, k, s=1, circ=False, relu=False, dtype=torch.float16, **kw):
+    return dict(Cout=cout, kh=k, kw=k, stride_h=s, stride_w=s, ph=k // 2, pw=k // 2, circ=circ, relu=relu,
+                out_dtype=dtype, **kw)
+
+
+def _caught_or_stray(exact, mutated, dtype):
+    """Like _caught, but a mutation that writes outside the contract's elements counts as caught too."""
+    ref, bound = exact
+    assert ct.worst_ratio(_kernel_like(ref, dtype), ref, bound) <= 1.0
+    try:
+        bad = ct.worst_ratio(_kernel_like(mutated, dtype), ref, bound)
+    except AssertionError:
+        return
+    assert bad > 1.0, bad
+
+
+@pytest.mark.parametrize("k,s,ph,pw", [(3, 1, 1, 1), (1, 2, 0, 0), (4, 2, 1, 1), (7, 2, 3, 3), (1, 1, 0, 0),
+                                       (3, 2, 0, 0), (5, 1, 2, 2)])
+@pytest.mark.parametrize("circ", [False, True])
+def test_conv_ref_matches_torch(k, s, ph, pw, circ):
+    """conv_ref against F.conv2d with explicit zero padding, or oracle.faed.circular_pad (rows zero, columns wrapped)."""
+    import torch.nn.functional as F
+    from oracle import faed as of
+    x, wp, bias, _ = _conv_operands(3 + k, B=2, H=9, W=8, cin=24, cout=10, k=k)
+    ref, bound = ct.conv_ref(x, wp, bias, Cout=10, kh=k, kw=k, stride_h=s, stride_w=s, ph=ph, pw=pw, circ=circ,
+                             relu=False, out_dtype=torch.float32)
+    w = wp.double()[:, :, :10].reshape(k, k, 32, 10).permute(3, 2, 0, 1)
+    xd = x.double().permute(0, 3, 1, 2)
+    y = F.conv2d(of.circular_pad(xd, ph) if circ else F.pad(xd, (pw, pw, ph, ph)), w, bias[:10].double(), stride=s)
+    assert torch.allclose(ref, y.permute(0, 2, 3, 1).reshape(-1, 10), rtol=1e-12, atol=1e-12)
+    assert (bound > 0).all()
+
+
+def test_conv_ref_stride_2_1_and_asymmetric_phase_pads():
+    """HorizonNet's (2, 1) stride, and a stride-2 data-gradient phase (2x2 kernel, pads (1 - r, 1 - c), Ho = H,
+    Wo = W given): both against F.conv2d on an explicitly padded input."""
+    import torch.nn.functional as F
+    from oracle import horizonnet as oh
+    x, wp, bias, _ = _conv_operands(11, H=8, W=6, cin=16, cin_pad=16, cout=8, k=3)
+    ref, _ = ct.conv_ref(x, wp, bias, Cout=8, kh=3, kw=3, stride_h=2, stride_w=1, ph=1, pw=1, circ=True, relu=False,
+                         out_dtype=torch.float32)
+    w = wp.double()[:, :, :8].reshape(3, 3, 16, 8).permute(3, 2, 0, 1)
+    y = oh.conv(x.double().permute(0, 3, 1, 2), w, bias[:8].double(), 3, (2, 1))
+    assert torch.allclose(ref, y.permute(0, 2, 3, 1).reshape(-1, 8), rtol=1e-12, atol=1e-12)
+    x, wp, bias, _ = _conv_operands(12, H=4, W=5, cin=16, cin_pad=16, cout=8, k=2)
+    w = wp.double()[:, :, :8].reshape(2, 2, 16, 8).permute(3, 2, 0, 1)
+    xd = x.double().permute(0, 3, 1, 2)
+    for r in (0, 1):
+        for c in (0, 1):
+            ref, _ = ct.conv_ref(x, wp, bias, Cout=8, kh=2, kw=2, stride_h=1, stride_w=1, ph=1 - r, pw=1 - c, circ=True,
+                                 relu=False, out_dtype=torch.float32, Ho=4, Wo=5)
+            xp = F.pad(torch.cat([xd[..., 5 - (1 - c):], xd, xd[..., :c]], -1), (0, 0, 1 - r, r))
+            y = F.conv2d(xp, w, bias[:8].double())
+            assert y.shape[-2:] == (4, 5)
+            assert torch.allclose(ref, y.permute(0, 2, 3, 1).reshape(-1, 8), rtol=1e-12, atol=1e-12), (r, c)
+
+
+def test_conv_ref_leaves_rows_past_m_and_columns_outside_the_slice_nan():
+    x, wp, bias, _ = _conv_operands(4, cout=6)
+    ref, bound = ct.conv_ref(x, wp, bias, **_conv_kw(6, 3, out_rows=70, out_ld=12, out_off=4))
+    M = 2 * 5 * 6
+    assert torch.isnan(ref[M:]).all() and torch.isnan(ref[:, :4]).all() and torch.isnan(ref[:, 10:]).all()
+    assert not torch.isnan(ref[:M, 4:10]).any() and torch.equal(torch.isnan(ref), torch.isnan(bound))
+
+
+CONV_DTYPES = [torch.float16, torch.float32]
+
+
+@pytest.mark.parametrize("dtype", CONV_DTYPES)
+def test_conv_seam_wrapped_to_zero_is_caught(dtype):
+    x, wp, bias, _ = _conv_operands(5, W=7, k=3, offset=0.5)
+    exact = ct.conv_ref(x, wp, bias, **_conv_kw(6, 3, circ=True, dtype=dtype))
+    mutated, _ = ct.conv_ref(x, wp, bias, **_conv_kw(6, 3, circ=False, dtype=dtype))
+    _caught(exact, mutated, dtype)
+
+
+@pytest.mark.parametrize("dtype", CONV_DTYPES)
+def test_conv_bias_of_the_neighbouring_column_is_caught(dtype):
+    x, wp, bias, _ = _conv_operands(6)
+    exact = ct.conv_ref(x, wp, bias, **_conv_kw(6, 3, relu=True, dtype=dtype))
+    b2 = bias.clone()
+    b2[1::2] = bias[0::2]  # the epilogue's column pair (c, c + 1) both take bias[c]
+    mutated, _ = ct.conv_ref(x, wp, b2, **_conv_kw(6, 3, relu=True, dtype=dtype))
+    _caught(exact, mutated, dtype)
+
+
+@pytest.mark.parametrize("dtype", CONV_DTYPES)
+def test_conv_dropped_last_k_chunk_of_a_tap_is_caught(dtype):
+    """Cin = 32 in two 16-channel k-steps per tap: the second chunk of tap 8 (the last k-step) is lost."""
+    x, wp, bias, _ = _conv_operands(7, cin=32, cin_pad=32)
+    exact = ct.conv_ref(x, wp, bias, **_conv_kw(6, 3, dtype=dtype))
+    w2 = wp.clone()
+    w2[8, 16:] = 0
+    mutated, _ = ct.conv_ref(x, w2, bias, **_conv_kw(6, 3, dtype=dtype))
+    _caught(exact, mutated, dtype)
+
+
+@pytest.mark.parametrize("dtype", CONV_DTYPES)
+def test_conv_residual_after_the_relu_is_caught(dtype):
+    x, wp, bias, res = _conv_operands(8, res=True)
+    exact = ct.conv_ref(x, wp, bias, **_conv_kw(6, 3, circ=True, relu=True, dtype=dtype, residual=res,
+                                                res_before_relu=True))
+    mutated, _ = ct.conv_ref(x, wp, bias, **_conv_kw(6, 3, circ=True, relu=True, dtype=dtype, residual=res))
+    _caught(exact, mutated, dtype)
+
+
+@pytest.mark.parametrize("dtype", CONV_DTYPES)
+def test_conv_tile_row_reading_the_previous_image_is_caught(dtype):
+    """The first output row of image 1 takes image 0's last input row for its top tap instead of zero padding: the
+    same convolution over the images stacked along H."""
+    x, wp, bias, _ = _conv_operands(9, B=3, H=4, W=6)
+    exact = ct.conv_ref(x, wp, bias, **_conv_kw(6, 3, circ=True, dtype=dtype))
+    mutated, _ = ct.conv_ref(x.reshape(1, 12, 6, 32), wp, bias, **_conv_kw(6, 3, circ=True, dtype=dtype))
+    assert torch.equal(mutated[:18], exact[0][:18])  # image 0's first three output rows are unchanged
+    _caught(exact, mutated, dtype)
+
+
+@pytest.mark.parametrize("dtype", CONV_DTYPES)
+def test_conv_column_past_cout_is_caught(dtype):
+    """FAED's last layer: Cout = 4 of a 32-wide packed weight; a store of column 4 (the next pair) fails."""
+    x, wp, bias, _ = _conv_operands(10, cout=3, cw=32, k=9, W=10)
+    exact = ct.conv_ref(x, wp, bias, **_conv_kw(4, 9, circ=True, dtype=dtype, out_ld=8))
+    assert torch.equal(exact[0][:, 3], bias[3].double().expand(exact[0].shape[0]))  # the zero weight column: bias only
+    mutated = exact[0].clone()
+    mutated[:, 4] = bias[4].double()
+    _caught_or_stray(exact, mutated, dtype)
+    with pytest.raises(AssertionError):
+        ct.worst_ratio(_kernel_like(mutated, dtype), *exact)
+
+
+@pytest.mark.parametrize("dtype", CONV_DTYPES)
+def test_conv_output_slice_shifted_by_two_columns_is_caught(dtype):
+    """An Inception branch written at out_off + 2 of its concat buffer."""
+    x, wp, bias, _ = _conv_operands(11, cout=10, cw=32)
+    exact = ct.conv_ref(x, wp, bias, **_conv_kw(10, 3, relu=True, dtype=dtype, out_ld=24, out_off=6))
+    mutated = torch.full_like(exact[0], float("nan"))
+    mutated[:, 8:18] = exact[0][:, 6:16]
+    _caught_or_stray(exact, mutated, dtype)
