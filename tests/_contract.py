@@ -18,6 +18,20 @@ element by about its own magnitude, far above the bound.
              convolution with the layer's own padding). ReLU is 1-Lipschitz and needs no factor. The deepest K any model
              passes is HorizonNet's first ConvCompressH, 9 * 2048 = 18432: sqrt(K) * 2^-24 = 8.1e-6, and ten times that
              rounds to the same power of two, 2^-14 (7.5x there, 9.5x at the tap-GEMM's 9 * 1280).
+  cpattn gather  |got - ref| <= 2^-21 * (sum_t w_t |x_t| + 1) + ulp_out(ref)  (pf_cpattn_gather, one key element: four
+             bilinear taps x_t with weights w_t, plus sin or cos of the fp32 product xy_rel * f). The weights carry <= 3
+             fp32 roundings (two subtractions, one product), the fma chain over the four taps <= 4, the PE add 1: 8 units
+             of 2^-24 = 2^-21 of the tap magnitude. sincosf is within 2 ulp of a value <= 1, 2^-22, under the "+ 1".
+             A masked key must be exactly zero (its bound is the smallest positive double).
+  cpattn stats   |got - ref| <= n * 2^-24 * (sum |k|, sum k^2) + 2^-60, n = 16 * ceil(C / 512) + 6, against the fp64
+             (sum, sum of squares) of the STORED 16-bit key row k: each lane adds 16 rounded values per 512 channels in
+             fp32, then five shuffle-tree adds.
+  cpattn attn    |got - ref| <= 2^-17 * (1 + A) * (P @ |V|) + ulp_out(ref)  (pf_cpattn_attn, one query against its 18
+             keys per 32-wide head). The kernel keeps P in fp32, so no 16-bit term enters before the output rounding.
+             A = scale * max_s sum_d |q_d k_sd| bounds the logits: the fp32 dot product errs by <= 33 units of 2^-24 * A
+             and a logit error e moves P by a relative 2e (66 A units); expf (2), the 18-term denominator (18), the
+             reciprocal and its product (2) and the 18-term fma chain of P V (18) add 40 units. 64 (1 + A) units is
+             2^-18 (1 + A); 2^-17 leaves a factor of two.
 
 Every function here runs on whichever device its inputs live on (the CPU tests use the same code at small sizes).
 """
@@ -213,6 +227,92 @@ def fmha_ref(q, k, v, *, heads: int, head_dim: int, scale: float, bias=None, chu
 def fmha_bound(ref, pv, dtype: torch.dtype):
     u = 2.0 ** -11 if dtype == torch.float16 else 2.0 ** -8
     return 2 * u * pv + u * ref.abs() + FMHA_FLOOR
+
+
+CP_SLOTS = 18
+GATHER_REL = 2.0 ** -21
+CPATTN_REL = 2.0 ** -17
+EXACT = torch.finfo(torch.float64).tiny  # bound of an element that must be exactly its reference
+
+
+def cpattn_gather_ref(x, B: int, m: int, h: int, w: int, C: int, G: int, pos, mask, freq, out_dtype: torch.dtype,
+                      neighbours=(-1, 1)):
+    """(ref, bound), fp64 [B * m * h * w * 18, C]: the key rows pf_cpattn_gather writes.
+
+    x: the [B * m * h * w, >= C] 16-bit tokens; pos fp32 [G, m, h * w, 18, 4] (grid_sample position in the neighbour's
+    map, xy_rel); mask uint8 [G, m, h * w, 18]; freq fp32 [C / 4]; G = 1 (every batch element shares the tables) or B.
+    Row ((b * m + i) * P + q) * 18 + s samples view i - 1 (s < 9) or i + 1 (ring order) of batch element b bilinearly
+    with zero padding (grid_sample, align_corners=True, at the unnormalised position) and adds
+    [sin(x f), sin(y f), cos(x f), cos(y f)] of the fp32-rounded products xy_rel * f, evaluated in fp64.
+    `neighbours` are the view offsets of slots 0-8 and 9-17."""
+    P = h * w
+    dev = x.device
+    xv = x[:, :C].reshape(B, m, P, C)
+    f32 = freq.float().reshape(-1)
+    N = C // 4
+    ref = torch.empty((B, m, P, CP_SLOTS, C), dtype=torch.float64, device=dev)
+    bound = torch.empty_like(ref)
+    side = torch.arange(CP_SLOTS, device=dev) < 9
+    for b in range(B):
+        g = 0 if G == 1 else b
+        for i in range(m):
+            p = pos[g, i].double()                                             # [P, 18, 4]
+            fx, fy = torch.floor(p[..., 0]), torch.floor(p[..., 1])
+            ax, ay = p[..., 0] - fx, p[..., 1] - fy
+            wts = ((1 - ax) * (1 - ay), ax * (1 - ay), (1 - ax) * ay, ax * ay)  # nw, ne, sw, se
+            acc = torch.zeros((P, CP_SLOTS, C), dtype=torch.float64, device=dev)
+            mag = torch.zeros_like(acc)
+            for t in range(4):
+                xx, yy = fx.long() + (t & 1), fy.long() + (t >> 1)
+                inside = (xx >= 0) & (xx < w) & (yy >= 0) & (yy < h)
+                idx = (yy.clamp(0, h - 1) * w + xx.clamp(0, w - 1))            # [P, 18]
+                left = xv[b, (i + neighbours[0]) % m].double()[idx]            # [P, 18, C]
+                right = xv[b, (i + neighbours[1]) % m].double()[idx]
+                val = torch.where(side[None, :, None], left, right)
+                wt = (wts[t] * inside)[..., None]
+                acc += wt * val
+                mag += wt * val.abs()
+            rel = pos[g, i, :, :, 2:].float()                                  # [P, 18, 2]
+            arg = (rel[..., :, None] * f32).double()                           # fp32 products, [P, 18, 2, N]
+            pe = torch.cat([arg.sin(), arg.cos()], -2).reshape(P, CP_SLOTS, 4 * N)
+            live = mask[g, i].bool()[..., None]
+            ref[b, i] = torch.where(live, acc + pe, 0.0)
+            bound[b, i] = GATHER_REL * (mag + 1.0)
+    ref = ref.reshape(-1, C)
+    bound = bound.reshape(-1, C) + ulp_out(ref, out_dtype)
+    masked = torch.stack([~mask[0 if G == 1 else b].bool() for b in range(B)]).reshape(-1)
+    bound[masked] = EXACT
+    return ref, bound
+
+
+def cpattn_stats_ref(keys, C: int):
+    """(ref, bound), fp64 [rows, 2]: (sum, sum of squares) of each stored 16-bit key row (pf_cpattn_gather's stats)."""
+    k = keys[:, :C].double()
+    n = 16 * -(-C // 512) + 6
+    ref = torch.stack([k.sum(1), (k * k).sum(1)], 1)
+    bound = n * 2.0 ** -24 * torch.stack([k.abs().sum(1), (k * k).sum(1)], 1) + 2.0 ** -60
+    return ref, bound
+
+
+def cpattn_attn_ref(q, kv, C: int, scale: float, out_dtype: torch.dtype, chunk: int = 4096):
+    """(ref, bound), fp64 [T, C]: pf_cpattn_attn, out[t, head] = softmax_s(q_t,head . k_ts,head * scale) v_ts,head over
+    the 18 key rows t * 18 + s of kv (K in columns [0, C), V in [C, 2C)), heads of width 32. Chunked over tokens."""
+    T, H = q.shape[0], C // 32
+    scale = float(torch.tensor(scale, dtype=torch.float32))
+    ref = torch.empty((T, C), dtype=torch.float64, device=q.device)
+    bound = torch.empty_like(ref)
+    for t0 in range(0, T, chunk):
+        t1 = min(T, t0 + chunk)
+        qh = q[t0:t1, :C].double().reshape(-1, H, 1, 32)
+        kvc = kv[t0 * CP_SLOTS:t1 * CP_SLOTS].double()
+        k = kvc[:, :C].reshape(-1, CP_SLOTS, H, 32).transpose(1, 2)          # [t, H, 18, 32]
+        v = kvc[:, C:2 * C].reshape(-1, CP_SLOTS, H, 32).transpose(1, 2)
+        s = (qh @ k.transpose(-1, -2)) * scale                                  # [t, H, 1, 18]
+        a = ((qh.abs() @ k.abs().transpose(-1, -2)) * scale).amax(-1, keepdim=True)
+        p = torch.softmax(s, -1)
+        ref[t0:t1] = (p @ v).reshape(-1, C)
+        bound[t0:t1] = (CPATTN_REL * (1.0 + a) * (p @ v.abs())).reshape(-1, C)
+    return ref, bound + ulp_out(ref, out_dtype)
 
 
 def worst_ratio(got, ref, bound) -> float:

@@ -288,3 +288,167 @@ def test_conv_output_slice_shifted_by_two_columns_is_caught(dtype):
     mutated = torch.full_like(exact[0], float("nan"))
     mutated[:, 8:18] = exact[0][:, 6:16]
     _caught_or_stray(exact, mutated, dtype)
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_causal_mask_shifted_by_one_key_is_caught(dtype):
+    """The text tower's causal bias (finfo(float32).min above the diagonal): one row that also sees the next key."""
+    g, q, k, v = _attention(dtype, 2, 9, 9, heads=2, d=64)
+    k, v = k[:, :9], v[:, :9]
+    causal = torch.full((9, 9), torch.finfo(torch.float32).min).triu(1)
+    ref, pv = ct.fmha_ref(q, k, v, heads=2, head_dim=64, scale=64 ** -0.5, bias=causal)
+    shifted = causal.clone()
+    shifted[4, 5] = 0.0
+    mutated, _ = ct.fmha_ref(q, k, v, heads=2, head_dim=64, scale=64 ** -0.5, bias=shifted)
+    _caught((ref, ct.fmha_bound(ref, pv, dtype)), mutated, dtype)
+
+
+# ---- correspondence-aware attention (cpattn.cu) ---------------------------------------------------------------------
+
+def _cp_rigs(B, m, img, G):
+    """K, R [B, m, 3, 3] of horizon rigs (FoV 120, so neighbouring views overlap): every element the same rig, or
+    (G = B) element b turned by 20 b degrees."""
+    import numpy as np
+    from oracle import mvdiffusion as omv
+    if G == 1:
+        return omv.horizon_cameras(m, batch=B, fov=120.0, size=img)
+    theta = np.rad2deg(np.linspace(0, 2 * np.pi, m, endpoint=False))
+    KR = [[omv.get_K_R(120.0, t + 20.0 * b, 0.0, img) for t in theta] for b in range(B)]
+    K = torch.stack([torch.from_numpy(np.stack([k for k, _ in row])) for row in KR])
+    R = torch.stack([torch.from_numpy(np.stack([r for _, r in row])) for row in KR])
+    return K, R
+
+
+def _cp_gather_setup(dtype, G=1, B=2, m=3, h=5, C=32, img=40, seed=12):
+    """Tokens [B * m * h * h, C] in the 16-bit type, the oracle's tables in pf_cpattn_tables' layout (pos | xy_rel) and
+    MVDiffusion's frequency table."""
+    from oracle import mvdiffusion as omv
+    from panfusion_b200.mvdiffusion import _PosEmbedding
+    K, R = _cp_rigs(B, m, img, G)
+    pos, mask, rel = omv.tables(K, R, h, img)
+    table = torch.cat([pos, rel], -1).float()[:G].contiguous()
+    x = torch.randn(B * m * h * h, C, generator=torch.Generator().manual_seed(seed)).to(dtype)
+    freq = _PosEmbedding(C // 4).freq_bands.reshape(-1).float()
+    return dict(x=x, B=B, m=m, h=h, w=h, C=C, G=G, pos=table, mask=mask[:G].to(torch.uint8), freq=freq), (pos, mask, rel)
+
+
+def test_cpattn_gather_ref_matches_the_oracle():
+    """cpattn_gather_ref equals oracle.mvdiffusion.gather_keys (F.grid_sample of the normalised grid + PosEmbedding,
+    times the mask) on the oracle's own tables, per batch element with its own cameras."""
+    from oracle import mvdiffusion as omv
+    kw, (pos, mask, rel) = _cp_gather_setup(torch.float16, G=2)
+    ref, bound = ct.cpattn_gather_ref(**kw, out_dtype=torch.float16)
+    B, m, h, C = kw["B"], kw["m"], kw["h"], kw["C"]
+    x5 = kw["x"].float().reshape(B, m, h, h, C).permute(0, 1, 4, 2, 3)
+    want = omv.gather_keys(x5, pos, mask, rel, kw["freq"]).reshape(-1, C)
+    assert mask.any() and not mask.all()
+    assert torch.allclose(ref, want.double(), rtol=0, atol=2e-5), (ref - want).abs().max()
+    assert (ref[~mask.reshape(-1)] == 0).all() and (bound > 0).all()
+
+
+def _gather_caught(kw, mutated, dtype):
+    ref, bound = ct.cpattn_gather_ref(**kw, out_dtype=dtype)
+    _caught((ref, bound), mutated, dtype)
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_cpattn_swapped_neighbours_are_caught(dtype):
+    kw, _ = _cp_gather_setup(dtype)
+    _gather_caught(kw, ct.cpattn_gather_ref(**kw, out_dtype=dtype, neighbours=(1, -1))[0], dtype)
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_cpattn_swapped_bilinear_weights_are_caught(dtype):
+    """The x fraction weighting the y taps and vice versa: the same taps at (floor x + frac y, floor y + frac x)."""
+    kw, _ = _cp_gather_setup(dtype)
+    p = kw["pos"].clone()
+    fx, fy = p[..., 0].floor(), p[..., 1].floor()
+    p[..., 0], p[..., 1] = fx + (kw["pos"][..., 1] - fy), fy + (kw["pos"][..., 0] - fx)
+    _gather_caught(kw, ct.cpattn_gather_ref(**dict(kw, pos=p), out_dtype=dtype)[0], dtype)
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_cpattn_swapped_pe_halves_are_caught(dtype):
+    kw, _ = _cp_gather_setup(dtype)
+    ref, _ = ct.cpattn_gather_ref(**kw, out_dtype=dtype)
+    N = kw["C"] // 4
+    arg = (kw["pos"][..., 2:, None] * kw["freq"]).double()            # [G, m, P, 18, 2, N]
+    sin, cos = arg.sin().flatten(-2), arg.cos().flatten(-2)
+    live = kw["mask"].bool().expand(kw["B"], -1, -1, -1).reshape(-1)
+    d = (torch.cat([cos - sin, sin - cos], -1)).expand(kw["B"], -1, -1, -1, -1).reshape(-1, 4 * N)
+    mutated = ref.clone()
+    mutated[live] += d[live]
+    _caught(ct.cpattn_gather_ref(**kw, out_dtype=dtype), mutated, dtype)
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_cpattn_unmasked_key_is_caught(dtype):
+    kw, _ = _cp_gather_setup(dtype)
+    ones = torch.ones_like(kw["mask"])
+    _gather_caught(kw, ct.cpattn_gather_ref(**dict(kw, mask=ones), out_dtype=dtype)[0], dtype)
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_cpattn_per_batch_tables_read_with_g0_are_caught(dtype):
+    kw, _ = _cp_gather_setup(dtype, G=2)
+    shared = dict(kw, G=1, pos=kw["pos"][:1], mask=kw["mask"][:1])
+    _gather_caught(kw, ct.cpattn_gather_ref(**shared, out_dtype=dtype)[0], dtype)
+
+
+def test_cpattn_stats_bound_accepts_fp32_sums_of_the_stored_keys():
+    kw, _ = _cp_gather_setup(torch.bfloat16, C=64)
+    ref, _ = ct.cpattn_gather_ref(**kw, out_dtype=torch.bfloat16)
+    keys = ref.to(torch.bfloat16)
+    k32 = keys.float()
+    got = torch.stack([k32.sum(1), (k32 * k32).sum(1)], 1).double()
+    want, bound = ct.cpattn_stats_ref(keys, 64)
+    assert ((got - want).abs() <= bound).all()
+    unrounded = torch.stack([ref.sum(1), (ref * ref).sum(1)], 1)      # statistics of the values before the store
+    assert ((unrounded - want).abs() > bound).any()
+
+
+def _cp_attn_setup(dtype, T=37, C=96, seed=13):
+    g = torch.Generator().manual_seed(seed)
+    q = (torch.randn(T, C, generator=g) * 2).to(dtype)
+    kv = torch.randn(T * 18, 2 * C, generator=g).to(dtype)
+    return q, kv
+
+
+def test_cpattn_attn_ref_matches_softmax_attention():
+    """cpattn_attn_ref equals the reference's attention (oracle.eppa's softmax(q k^T * scale) v per head) over the
+    18 keys of each query; below the output rounding its bound is at least four times tighter than fmha_bound."""
+    q, kv = _cp_attn_setup(torch.float16)
+    T, C = q.shape
+    ref, bound = ct.cpattn_attn_ref(q, kv, C, 32 ** -0.5, torch.float16)
+    sc = float(torch.tensor(32 ** -0.5, dtype=torch.float32))  # the kernel's float argument
+    qh = q.double().reshape(T, 1, C // 32, 32).transpose(1, 2)
+    k = kv[:, :C].double().reshape(T, 18, C // 32, 32).transpose(1, 2)
+    v = kv[:, C:].double().reshape(T, 18, C // 32, 32).transpose(1, 2)
+    want = (torch.softmax(qh @ k.transpose(-1, -2) * sc, -1) @ v).transpose(1, 2).reshape(T, C)
+    assert torch.allclose(ref, want, rtol=1e-12, atol=1e-12)
+    pv = (torch.softmax(qh @ k.transpose(-1, -2) * sc, -1) @ v.abs()).transpose(1, 2).reshape(T, C)
+    loose = ct.fmha_bound(ref, pv, torch.float16)
+    assert (bound - ct.ulp_out(ref, torch.float16) < loose / 4).all()
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_cpattn_dropped_key_slot_is_caught(dtype):
+    """The softmax over 17 of the 18 slots (the last one never read)."""
+    q, kv = _cp_attn_setup(dtype)
+    T, C = q.shape
+    exact = ct.cpattn_attn_ref(q, kv, C, 32 ** -0.5, dtype)
+    qh = q.double().reshape(T, 1, C // 32, 32).transpose(1, 2)
+    k = kv[:, :C].double().reshape(T, 18, C // 32, 32).transpose(1, 2)[:, :, :17]
+    v = kv[:, C:].double().reshape(T, 18, C // 32, 32).transpose(1, 2)[:, :, :17]
+    mutated = (torch.softmax(qh @ k.transpose(-1, -2) * 32 ** -0.5, -1) @ v).transpose(1, 2).reshape(T, C)
+    _caught(exact, mutated, dtype)
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_cpattn_head_reading_the_next_heads_v_is_caught(dtype):
+    q, kv = _cp_attn_setup(dtype)
+    C = q.shape[1]
+    exact = ct.cpattn_attn_ref(q, kv, C, 32 ** -0.5, dtype)
+    kv2 = kv.clone()
+    kv2[:, C:] = kv[:, C:].roll(-32, 1)  # head h's V columns hold head h + 1's
+    _caught(exact, ct.cpattn_attn_ref(q, kv2, C, 32 ** -0.5, dtype)[0], dtype)
