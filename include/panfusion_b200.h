@@ -259,9 +259,11 @@ int pf_conv_prep(const void* x, void* out, int dtype, int N, int H, int W, int C
  *   statistics over the image circularly extended by circ_stats columns (duplicated columns count twice), applied with
  *   gamma / beta (+ SiLU) while building the conv_prep layout (circ, up, phases, halo as in pf_conv_prep).
  * Two launches: the statistics with one CTA per slab of each image, then the apply pass with up to 64 CTAs per image (the
- * source is re-read from L2). ws: pf_gn_prep_ws_floats(N, groups) floats of scratch; counters: N ints that are ZERO on
- * entry (restored to zero by the kernel; concurrent launches need distinct slots). The partition of every sum depends on
- * H*W only, never on N: results are bit-identical for any batch size. */
+ * source is re-read from L2). ws: pf_gn_prep_ws_floats(N, groups) floats of scratch: N * 64 * groups * 2 partial sums,
+ * then the statistics the apply launch reads, mean_rstd [N, groups, 2] fp32 at ws + N * 64 * groups * 2 (as
+ * pf_groupnorm_stats writes them; they stay there after the call). counters: N ints that are ZERO on entry (restored to
+ * zero by the kernel; concurrent launches need distinct slots). The partition of every sum depends on H*W only, never on
+ * N: results are bit-identical for any batch size. */
 int pf_gn_prep_ws_floats(int N, int groups);
 int pf_gn_prep(const void* x1, int ld1, int C1, const void* x2, int ld2, int C2, void* cat_out, void* out, int dtype,
                int N, int H, int W, int groups, float eps, const float* gamma, const float* beta, int act,

@@ -33,6 +33,37 @@ element by about its own magnitude, far above the bound.
              reciprocal and its product (2) and the 18-term fma chain of P V (18) add 40 units. 64 (1 + A) units is
              2^-18 (1 + A); 2^-17 leaves a factor of two.
 
+The normalisation and sampler kernels (csrc/norm.cu, csrc/elementwise.cu), u = 2^-24:
+  gn stats   (pf_groupnorm_stats, the statistics launch of pf_gn_prep) mean and rstd of each (image, group) over the image
+             circularly extended by circ_stats columns, a duplicated column weighted w = 2 (3 when both seams cover it).
+             w x and w x^2 are exact in fp32 (a 16-bit x has <= 11 significant bits, w <= 2 bits), so only additions
+             round: a thread adds ceil(ceil(HW / slabs) / ppi) pixels, the CTA adds its ppi lanes, then cpg channels, all
+             in fp32; slabs are added in fp64. With n = ceil(ceil(HW / slabs) / ppi) + ppi + cpg, S1 = sum w |x| and
+             S2 = sum w x^2 over `count` = H (W + 2 circ_stats) cpg terms:
+               |dmean| <= n u S1 / count + u |mean|                       (the fp32 store adds the last term)
+               dvar    <= n u S2 / count + 2 |mean| n u S1 / count <= 3 n u S2 / count   ((S1 / count)^2 <= S2 / count)
+               |drstd| / rstd <= 1/2 * 3 n u (S2 / count) / (var + eps) + 2u   (fp64 sqrt and the fp32 store)
+             This is the one-pass form the kernel computes; for a near-constant group the bound is vacuous by design.
+  gn apply   (pf_conv_prep / the apply launch of pf_gn_prep) y = x sc + sh with sc = fl(rstd gamma), sh = fl(beta - mean sc)
+             from the fp32 (mean, rstd) the launch reads: four roundings of the x term, four of the mean term and two
+             of beta: |dy| <= 4u ((|x| + |mean|) rstd |gamma| + |beta|) (sh carries the cancellation, so the bound is
+             not on |x - mean|). SiLU (silu_f: ex2.approx, rcp.approx, <= 2 ulp each, the argument's product and the
+             final product) adds 1.13 |dy| + 2^-20 (1 + |y|) |silu(y)|. Halo and phase padding, the raw concatenation
+             and conv_prep without statistics are exact.
+  layernorm  (pf_layernorm) f = fl(x + pe), then the two-pass fp32 form in one warp: each lane adds 8 ceil(C / 256)
+             values, then 5 shuffles: n = 8 ceil(C / 256) + 5, dmean <= n u sum|f| / C + u |mean|; the squares carry
+             (n + 4) u of var (d = f - mean rounds, d^2 rounds, the sum, / C) plus the (dmean)^2 / var the shifted centre
+             adds, + eps rounds once, rsqrtf is within 2 ulp (4u): drstd / rstd <= 1/2 (n + 5) u var / (var + eps) +
+             dmean^2 / (2 (var + eps)) + 4u. Output: |do| <= |gamma| rstd (dmean + |f - mean| (3u + drstd / rstd)) +
+             u |o|, then the 16-bit store.
+  row stats  (pf_embed_tokens) the row is exactly fl16(fl32(tok[id] + pos[t % L])); its (sum, sum of squares) as the
+             cpattn stats with n = 2 ceil(C / 64) + 5 (a lane adds a pair, then the pair to its sum, per 64 channels).
+  cfg ddim   (pf_cfg_ddim_step[_dev]) e = eu + g (ec - eu), v = c_x x + c_eps e in fp32, stored at column (col + roll) mod
+             W: |dv| <= 2u (|c_x x| + 2 |c_eps e| + 2 |c_eps g (ec - eu)| + |v|) (first order, doubled).
+  timestep   (pf_timestep_embed) [cos(t f_i) | sin(t f_i)], f_i = 10000^(-i / half). The fp32 argument t f_i carries
+             logf (2u), two products (2u) and expf (4u) of ln f_i, then the product by t: |darg| <= u (4 |ln f_i| + 5)
+             |t f_i|; cosf / sinf add 2 ulp of a value <= 1 (2^-22).
+
 Every function here runs on whichever device its inputs live on (the CPU tests use the same code at small sizes).
 """
 from __future__ import annotations
@@ -285,13 +316,17 @@ def cpattn_gather_ref(x, B: int, m: int, h: int, w: int, C: int, G: int, pos, ma
     return ref, bound
 
 
+def _row_sums(rows, n: int):
+    """(ref, bound), fp64 [rows, 2]: (sum, sum of squares) of 16-bit rows summed in fp32 chains of n additions."""
+    k = rows.double()
+    ref = torch.stack([k.sum(1), (k * k).sum(1)], 1)
+    bound = n * U * torch.stack([k.abs().sum(1), (k * k).sum(1)], 1) + 2.0 ** -60
+    return ref, bound
+
+
 def cpattn_stats_ref(keys, C: int):
     """(ref, bound), fp64 [rows, 2]: (sum, sum of squares) of each stored 16-bit key row (pf_cpattn_gather's stats)."""
-    k = keys[:, :C].double()
-    n = 16 * -(-C // 512) + 6
-    ref = torch.stack([k.sum(1), (k * k).sum(1)], 1)
-    bound = n * 2.0 ** -24 * torch.stack([k.abs().sum(1), (k * k).sum(1)], 1) + 2.0 ** -60
-    return ref, bound
+    return _row_sums(keys[:, :C], 16 * -(-C // 512) + 6)
 
 
 def cpattn_attn_ref(q, kv, C: int, scale: float, out_dtype: torch.dtype, chunk: int = 4096):
@@ -313,6 +348,163 @@ def cpattn_attn_ref(q, kv, C: int, scale: float, out_dtype: torch.dtype, chunk: 
         ref[t0:t1] = (p @ v).reshape(-1, C)
         bound[t0:t1] = (CPATTN_REL * (1.0 + a) * (p @ v.abs())).reshape(-1, C)
     return ref, bound + ulp_out(ref, out_dtype)
+
+
+U = 2.0 ** -24
+SILU_REL = 2.0 ** -20
+
+
+def _f32(v: float) -> float:
+    """A Python float as the kernel receives it (a C float argument)."""
+    return float(torch.tensor(v, dtype=torch.float32))
+
+
+def gn_partition(entry: str, H: int, W: int, C: int):
+    """(slabs, ppi) of the statistics launch: pf_gn_prep cuts an image into <= 32 slabs of >= 16 pixels with 512-thread
+    CTAs, pf_groupnorm_stats into <= 64 with 256-thread CTAs; a CTA covers ppi pixels per step (C / 8 lanes each)."""
+    threads, cap = (512, 32) if entry == "pf_gn_prep" else (256, 64)
+    return min(max(H * W // 16, 1), cap), max(1, threads // (C // 8))
+
+
+def gn_operand(g, N: int, H: int, W: int, C: int, groups: int, dtype: torch.dtype, seam: int = 2):
+    """Channels-last tokens [N * H * W, C] that make GroupNorm indexing bugs visible: each (image, group) has its own
+    scale s in [0.5, 2] and offset in [-4 s, 4 s], and the `seam` columns at either edge are shifted by +s (left) and
+    -s (right), so the two sides of the circular seam differ."""
+    cpg = C // groups
+    s = (0.5 + 1.5 * torch.rand(N, 1, 1, groups, 1, generator=g))
+    off = s * (8 * torch.rand(N, 1, 1, groups, 1, generator=g) - 4)
+    x = torch.randn(N, H, W, groups, cpg, generator=g) * s + off
+    if seam:
+        x[:, :, :min(seam, W)] += s
+        x[:, :, max(0, W - seam):] -= s
+    return x.reshape(N * H * W, C).to(dtype)
+
+
+def gn_stats_ref(x, N: int, H: int, W: int, groups: int, circ_stats: int, eps: float, partition):
+    """(ref, bound), fp64 [N, groups, 2]: GroupNorm (mean, rstd) of x [N * H * W, C] (the concatenation, channels
+    last) over each image circularly extended by circ_stats columns; `partition` = gn_partition(...)."""
+    slabs, ppi = partition
+    C = x.shape[1]
+    cpg, hw = C // groups, H * W
+    n = -(-(-(-hw // slabs)) // ppi) + ppi + cpg
+    col = torch.arange(W, device=x.device)
+    w = (1.0 + (col < circ_stats).double() + (col >= W - circ_stats).double())[None, :, None, None]
+    count = H * (W + 2 * circ_stats) * cpg
+    eps = _f32(eps)
+    ref = torch.empty((N, groups, 2), dtype=torch.float64, device=x.device)
+    bound = torch.empty_like(ref)
+    for b in range(N):
+        xb = x[b * hw:(b + 1) * hw].double().reshape(H, W, groups, cpg)
+        s1 = (w * xb).sum((0, 1, 3))
+        a1 = (w * xb.abs()).sum((0, 1, 3))
+        s2 = (w * xb * xb).sum((0, 1, 3))
+        mean = s1 / count
+        var = (w * (xb - mean[None, None, :, None]) ** 2).sum((0, 1, 3)) / count
+        rstd = 1.0 / torch.sqrt(var + eps)
+        ref[b, :, 0], ref[b, :, 1] = mean, rstd
+        bound[b, :, 0] = n * U * a1 / count + U * mean.abs()
+        bound[b, :, 1] = rstd * (1.5 * n * U * (s2 / count) / (var + eps) + 2 * U)
+        del xb
+    return ref, bound
+
+
+def _layout(t, circ: int, up: int, phases: int, halo: int, fill: float):
+    """[N, H, W, C] -> the pf_conv_prep layout [phases * N * Ho * Wo, C], `fill` in the halo / phase padding."""
+    W = t.shape[2]
+    if circ:
+        t = t[:, :, (torch.arange(W + 2 * circ, device=t.device) - circ) % W]
+    if up > 1:
+        t = t.repeat_interleave(up, 1).repeat_interleave(up, 2)
+    pad = 1 if phases == 4 else halo
+    t = torch.nn.functional.pad(t, (0, 0, pad, pad, pad, pad), value=fill)
+    if phases == 4:
+        t = torch.stack([t[:, py::2, px::2] for py in (0, 1) for px in (0, 1)])
+    return t.reshape(-1, t.shape[-1])
+
+
+def gn_apply_ref(x, N: int, H: int, W: int, mean_rstd, gamma, beta, *, act: int, circ: int, up: int, phases: int,
+                 halo: int, out_dtype: torch.dtype):
+    """(ref, bound), fp64 [phases * N * Ho * Wo, C]: pf_conv_prep (and pf_gn_prep's apply launch) on x [N * H * W, C]
+    with the fp32 mean_rstd [N, groups, 2] the launch reads (None: no normalisation, the layout alone is exact).
+    Halo and phase-padding positions must be exactly zero."""
+    C = x.shape[1]
+    y = x.double().reshape(N, H, W, C)
+    if mean_rstd is None:
+        assert act == ACT_NONE
+        dy = torch.full_like(y, EXACT)
+    else:
+        cpg = C // mean_rstd.shape[1]
+        mr = mean_rstd.double().repeat_interleave(cpg, 1)[:, None, None]     # [N, 1, 1, C, 2]
+        mean, rstd = mr[..., 0], mr[..., 1]
+        g, b = gamma.double(), beta.double()
+        dy = 4 * U * ((y.abs() + mean.abs()) * rstd * g.abs() + b.abs())
+        y = (y - mean) * rstd * g + b
+        if act == ACT_SILU:
+            s = _silu(y)
+            dy = ACT_LIP * dy + SILU_REL * (1.0 + y.abs()) * s.abs()
+            y = s
+        dy = dy + ulp_out(y, out_dtype)
+    return _layout(y, circ, up, phases, halo, 0.0), _layout(dy, circ, up, phases, halo, EXACT)
+
+
+def layernorm_ref(x, pe, gamma, beta, eps: float, out_dtype: torch.dtype, chunk: int = 1 << 15):
+    """(ref, bound), fp64 [T, C]: pf_layernorm, LayerNorm(fl32(x[t] + pe[t % pe_rows])) * gamma + beta for the rows of
+    the 16-bit view x [T, C] (any row stride); pe fp32 [pe_rows, C] or None."""
+    T, C = x.shape
+    n = 8 * -(-C // 256) + 5
+    eps = _f32(eps)
+    g, b = gamma.double(), beta.double()
+    ref = torch.empty((T, C), dtype=torch.float64, device=x.device)
+    bound = torch.empty_like(ref)
+    for t0 in range(0, T, chunk):
+        t1 = min(T, t0 + chunk)
+        f = x[t0:t1].float()
+        if pe is not None:
+            f = f + pe[torch.arange(t0, t1, device=x.device) % pe.shape[0]]  # the fp32 add the kernel does
+        f = f.double()
+        mean = f.mean(1, keepdim=True)
+        d = f - mean
+        var = (d * d).mean(1, keepdim=True)
+        rstd = 1.0 / torch.sqrt(var + eps)
+        o = d * rstd * g + b
+        dmean = n * U * f.abs().mean(1, keepdim=True) + U * mean.abs()
+        rel = 0.5 * (n + 5) * U * var / (var + eps) + dmean ** 2 / (2 * (var + eps)) + 4 * U
+        ref[t0:t1] = o
+        bound[t0:t1] = g.abs() * rstd * (dmean + d.abs() * (3 * U + rel)) + U * o.abs() + ulp_out(o, out_dtype)
+    return ref, bound
+
+
+def row_stats_ref(tok, pos, ids, L: int, out_dtype: torch.dtype):
+    """pf_embed_tokens -> (row [T, C] in out_dtype, exact: fl16(fl32(tok[id] + pos[t % L]))), then (ref, bound) fp64
+    [T, 2] of the (sum, sum of squares) of that stored row."""
+    T, C = ids.numel(), tok.shape[1]
+    row = (tok[ids] + pos[torch.arange(T, device=ids.device) % L]).to(out_dtype)
+    return (row, *_row_sums(row, 2 * -(-C // 64) + 5))
+
+
+def cfg_ddim_ref(x, eps, coef, guidance: float, roll: int):
+    """(ref, bound), fp64 shaped like x: pf_cfg_ddim_step[_dev] on x fp32 [..., W], eps [uncond | text] with 2 x.numel()
+    elements, coef fp32 (c_x, c_eps) as the sampler's coef_table holds them; element (.., col) goes to column
+    (col + roll) mod W."""
+    W = x.shape[-1]
+    xr = x.double().reshape(-1, W)
+    eu, ec = eps.double().reshape(2, -1, W).unbind(0)
+    g = _f32(guidance)
+    cx, ce = (float(c) for c in coef.double().cpu())
+    e = eu + g * (ec - eu)
+    v = cx * xr + ce * e
+    bound = 2 * U * ((cx * xr).abs() + 2 * (ce * e).abs() + 2 * (ce * g * (ec - eu)).abs() + v.abs()) + EXACT
+    return v.roll(roll, -1).reshape(x.shape), bound.roll(roll, -1).reshape(x.shape)
+
+
+def timestep_ref(t, dim: int, out_dtype: torch.dtype):
+    """(ref, bound), fp64 [n, dim]: diffusers Timesteps(dim, flip_sin_to_cos=True, freq_shift=0) of t fp32 [n]."""
+    half = dim // 2
+    lnf = -math.log(10000.0) * torch.arange(half, dtype=torch.float64, device=t.device) / half
+    arg = t.double()[:, None] * torch.exp(lnf)
+    ref = torch.cat([arg.cos(), arg.sin()], 1)
+    b = U * (4 * lnf.abs() + 5) * arg.abs() + 2.0 ** -22
+    return ref, torch.cat([b, b], 1) + ulp_out(ref, out_dtype)
 
 
 def worst_ratio(got, ref, bound) -> float:

@@ -6,7 +6,11 @@ row-bias group, a halo row in the output, a residual read one row off, swapped G
 bias read from the wrong batch) and checks that the bound catches it on at least one element. The convolution cases
 (conv_ref, the contract of csrc/conv_mma.cuh) first pin conv_ref to F.conv2d, then emulate a seam column wrapped to
 zero, a neighbouring column's bias, a dropped K chunk, the residual on the wrong side of the ReLU, a tile row reading the
-previous image, a store past Cout and a shifted output slice."""
+previous image, a store past Cout and a shifted output slice. The normalisation and sampler references (GroupNorm,
+LayerNorm, the token embedding's row statistics, CFG + DDIM, the timestep embedding) are pinned to F.group_norm on
+pad_pano, F.layer_norm, the oracle's DDIM step and Timesteps, then shown to catch a dropped pixel, a one-sided seam
+weight, a count over the unpadded width, the next group's or another image's statistics, a block-indexed PE, a skipped
+token, a reversed roll, swapped CFG halves, swapped sin / cos halves and statistics of the unrounded row."""
 import pytest
 import torch
 
@@ -452,3 +456,210 @@ def test_cpattn_head_reading_the_next_heads_v_is_caught(dtype):
     kv2 = kv.clone()
     kv2[:, C:] = kv[:, C:].roll(-32, 1)  # head h's V columns hold head h + 1's
     _caught(exact, ct.cpattn_attn_ref(q, kv2, C, 32 ** -0.5, dtype)[0], dtype)
+
+
+# ---- normalisation and sampler kernels (norm.cu, elementwise.cu) ---------------------------------------------------
+
+def _nchw(x, N, H, W):
+    return x.double().reshape(N, H, W, -1).permute(0, 3, 1, 2)
+
+
+def _gn_setup(dtype, N=2, H=4, W=12, C=64, groups=32, seed=20):
+    g = torch.Generator().manual_seed(seed)
+    x = ct.gn_operand(g, N, H, W, C, groups, dtype)
+    return x, torch.randn(C, generator=g), torch.randn(C, generator=g)
+
+
+@pytest.mark.parametrize("circ_stats,circ,phases,up,halo,act", [
+    (2, 2, 1, 1, 1, ct.ACT_SILU),   # panorama norm1: pad_pano(2) statistics and layout
+    (0, 1, 1, 1, 1, ct.ACT_SILU),   # conv_out: statistics of the unpadded tensor, pad_pano(1) layout
+    (0, 0, 1, 1, 0, ct.ACT_NONE),   # the transformer's plain GroupNorm
+    (2, 2, 4, 1, 1, ct.ACT_SILU),   # stride-2 phases
+    (1, 1, 1, 2, 1, ct.ACT_SILU),   # nearest x2
+])
+def test_gn_refs_match_torch_group_norm(circ_stats, circ, phases, up, halo, act):
+    """gn_stats_ref and gn_apply_ref equal F.group_norm of pad_pano(x, circ_stats) applied to pad_pano(x, circ), then
+    SiLU, nearest x2, the zero halo and the stride-2 phase split (the composition of the reference's modules)."""
+    import torch.nn.functional as F
+    from oracle.eppa import pad_pano
+    N, H, W, C, G = 2, 4, 12, 64, 32
+    x, gamma, beta = _gn_setup(torch.float16, N, H, W, C, G)
+    xs = pad_pano(_nchw(x, N, H, W), circ_stats)
+    mean = xs.reshape(N, G, -1).mean(-1)
+    rstd = (xs.reshape(N, G, -1).var(-1, unbiased=False) + ct._f32(1e-5)).rsqrt()
+    stats, sb = ct.gn_stats_ref(x, N, H, W, G, circ_stats, 1e-5, ct.gn_partition("pf_gn_prep", H, W, C))
+    assert torch.allclose(stats[..., 0], mean, rtol=1e-12, atol=1e-12)
+    assert torch.allclose(stats[..., 1], rstd, rtol=1e-12, atol=1e-12)
+    assert (sb > 0).all()
+    full = F.group_norm(pad_pano(_nchw(x, N, H, W), circ), G, gamma.double(), beta.double(), 1e-5)
+    if circ_stats != circ:  # the statistics come from the other width: apply them by hand
+        cpg = C // G
+        full = ((pad_pano(_nchw(x, N, H, W), circ) - mean.repeat_interleave(cpg, 1)[..., None, None])
+                * rstd.repeat_interleave(cpg, 1)[..., None, None] * gamma.double()[:, None, None] + beta.double()[:, None, None])
+    if act == ct.ACT_SILU:
+        full = F.silu(full)
+    if up == 2:
+        full = F.interpolate(full, scale_factor=2.0, mode="nearest")
+    full = F.pad(full, [1, 1, 1, 1]) if (halo or phases == 4) else full
+    if phases == 4:
+        want = torch.stack([full[:, :, py::2, px::2] for py in (0, 1) for px in (0, 1)]).permute(0, 1, 3, 4, 2)
+    else:
+        want = full.permute(0, 2, 3, 1)
+    ref, bound = ct.gn_apply_ref(x, N, H, W, stats.float(), gamma, beta, act=act, circ=circ, up=up, phases=phases,
+                                 halo=halo, out_dtype=torch.float16)
+    # the reference applies fp64 statistics, the contract the fp32 ones the launch reads
+    assert torch.allclose(ref, want.reshape(ref.shape), rtol=1e-6, atol=1e-6)
+    pad = (want.reshape(ref.shape) == 0).all(1)
+    assert pad.any() == bool(halo or phases == 4) and (bound[pad] == ct.EXACT).all() and (ref[pad] == 0).all()
+
+
+def _stats(x, N, H, W, G, weights, count, eps=1e-5):
+    """fp64 (mean, rstd) of x with per-column weights and an explicit count: the emulated statistics bugs."""
+    cpg = x.shape[1] // G
+    xb = x.double().reshape(N, H, W, G, cpg)
+    w = weights.double()[None, None, :, None, None]
+    mean = (w * xb).sum((1, 2, 4)) / count
+    var = (w * xb * xb).sum((1, 2, 4)) / count - mean * mean
+    return torch.stack([mean, 1.0 / torch.sqrt(var + ct._f32(eps))], -1)
+
+
+def _seam_weights(W, circ, left=True, right=True):
+    col = torch.arange(W)
+    return 1.0 + left * (col < circ).double() + right * (col >= W - circ).double()
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+@pytest.mark.parametrize("bug", ["dropped pixel", "one-sided seam", "unpadded count"])
+def test_gn_stats_bugs_are_caught(dtype, bug):
+    """One pixel of a slab never added; the duplicated seam columns weighted on the left side only; the count taken
+    over the unpadded width. Shapes as the UNet's panorama norm1 at a small level (pad_pano(2) statistics)."""
+    N, H, W, C, G, circ = 2, 8, 16, 128, 32, 2
+    x, _, _ = _gn_setup(dtype, N, H, W, C, G, seed=21)
+    exact = ct.gn_stats_ref(x, N, H, W, G, circ, 1e-5, ct.gn_partition("pf_gn_prep", H, W, C))
+    count = H * (W + 2 * circ) * (C // G)
+    if bug == "dropped pixel":
+        xd = x.clone()
+        xd[(H * W) // 2 + 3] = 0  # a pixel inside a slab of image 0
+        mutated = _stats(xd, N, H, W, G, _seam_weights(W, circ), count)
+    elif bug == "one-sided seam":
+        mutated = _stats(x, N, H, W, G, _seam_weights(W, circ, right=False), count)
+    else:
+        mutated = _stats(x, N, H, W, G, _seam_weights(W, circ), H * W * (C // G))
+    assert torch.allclose(_stats(x, N, H, W, G, _seam_weights(W, circ), count), exact[0], rtol=1e-9, atol=1e-9)
+    _caught(exact, mutated, torch.float32)
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+@pytest.mark.parametrize("bug", ["next group", "other image"])
+def test_gn_apply_bugs_are_caught(dtype, bug):
+    """A group-edge channel normalised with the next group's statistics; an image normalised with another's."""
+    N, H, W, C, G = 2, 4, 8, 128, 32
+    x, gamma, beta = _gn_setup(dtype, N, H, W, C, G, seed=22)
+    st = ct.gn_stats_ref(x, N, H, W, G, 0, 1e-5, ct.gn_partition("pf_gn_prep", H, W, C))[0].float()
+    kw = dict(act=ct.ACT_SILU, circ=0, up=1, phases=1, halo=1, out_dtype=dtype)
+    exact = ct.gn_apply_ref(x, N, H, W, st, gamma, beta, **kw)
+    if bug == "next group":
+        mutated = exact[0].clone()
+        edge = C // G - 1  # the last channel of group 0
+        mutated[:, edge] = ct.gn_apply_ref(x, N, H, W, st.roll(-1, 1), gamma, beta, **kw)[0][:, edge]
+    else:
+        mutated = ct.gn_apply_ref(x, N, H, W, st.roll(1, 0), gamma, beta, **kw)[0]
+    _caught(exact, mutated, dtype)
+
+
+def _ln_setup(dtype, T=64, C=320, pe_rows=16, seed=23):
+    g = torch.Generator().manual_seed(seed)
+    x = (torch.randn(T, C, generator=g) * 2 + 0.5).to(dtype)
+    pe = torch.randn(pe_rows, C, generator=g)
+    return x, pe, torch.randn(C, generator=g), torch.randn(C, generator=g)
+
+
+def test_layernorm_ref_matches_torch_layer_norm():
+    import torch.nn.functional as F
+    x, pe, gamma, beta = _ln_setup(torch.bfloat16)
+    ref, bound = ct.layernorm_ref(x, pe, gamma, beta, 1e-5, torch.bfloat16)
+    f = (x.float() + pe.repeat(x.shape[0] // pe.shape[0], 1)).double()
+    want = F.layer_norm(f, (x.shape[1],), gamma.double(), beta.double(), ct._f32(1e-5))
+    assert torch.allclose(ref, want, rtol=1e-12, atol=1e-12) and (bound > 0).all()
+    ref0, _ = ct.layernorm_ref(x[::2], None, gamma, beta, 1e-5, torch.bfloat16)  # a strided view, no PE
+    assert torch.allclose(ref0, F.layer_norm(x[::2].double(), (x.shape[1],), gamma.double(), beta.double(), ct._f32(1e-5)))
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+@pytest.mark.parametrize("bug", ["pe by block", "skipped token"])
+def test_layernorm_bugs_are_caught(dtype, bug):
+    """pe[t // (T / pe_rows)] instead of pe[t % pe_rows]; the second token of a warp never written (NaN-filled)."""
+    x, pe, gamma, beta = _ln_setup(dtype)
+    exact = ct.layernorm_ref(x, pe, gamma, beta, 1e-5, dtype)
+    T, rows = x.shape[0], pe.shape[0]
+    if bug == "pe by block":
+        mutated, _ = ct.layernorm_ref(x, pe[torch.arange(T) // (T // rows)], gamma, beta, 1e-5, dtype)
+    else:
+        mutated = exact[0].clone()
+        mutated[1] = float("nan")
+    _caught(exact, mutated, dtype)
+
+
+def _embed_setup(T=154, L=77, C=192, vocab=50, seed=24):
+    g = torch.Generator().manual_seed(seed)
+    return (torch.randn(vocab, C, generator=g) * 0.5 + 0.1, torch.randn(L, C, generator=g) * 0.3,
+            torch.randint(0, vocab, (T,), generator=g), L)
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_row_stats_of_the_fp32_row_are_caught(dtype):
+    """The statistics must be those of the stored 16-bit row: fp32 sums of it pass, the unrounded row's fail."""
+    tok, pos, ids, L = _embed_setup()
+    row, ref, bound = ct.row_stats_ref(tok, pos, ids, L, dtype)
+    assert torch.equal(row, (tok[ids] + pos.repeat(2, 1)).to(dtype))
+    r32 = row.float()
+    got = torch.stack([r32.sum(1), (r32 * r32).sum(1)], 1).double()
+    assert ((got - ref).abs() <= bound).all()
+    f = (tok[ids] + pos.repeat(2, 1)).double()
+    assert ((torch.stack([f.sum(1), (f * f).sum(1)], 1) - ref).abs() > bound).any()
+
+
+def _ddim_setup(seed=25, W=32):
+    from panfusion_b200.sampler import DDIMSchedule
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(2, 4, 16, W, generator=g)
+    eps = torch.randn(2, 2, 4, 16, W, generator=g)
+    sched = DDIMSchedule()
+    sched.set_timesteps(50)
+    t = int(sched.timesteps[3])
+    return x, eps, t, torch.tensor(sched.coefficients(t), dtype=torch.float32)
+
+
+def test_cfg_ddim_ref_matches_the_oracle_step():
+    """cfg_ddim_ref with the sampler's fp32 coefficients equals the oracle's CFG combine + DDIM step, rolled."""
+    from oracle.sampler import DDIM
+    x, eps, t, coef = _ddim_setup()
+    sched = DDIM()
+    sched.set_timesteps(50)
+    e = eps[0].double() + 9.0 * (eps[1].double() - eps[0].double())
+    want = torch.roll(sched.step(e, t, x.double()), 8, dims=-1)
+    ref, bound = ct.cfg_ddim_ref(x, eps, coef, 9.0, 8)
+    assert torch.allclose(ref, want, rtol=0, atol=2e-6)  # the coefficients are fp32
+    assert (bound > 0).all()
+
+
+@pytest.mark.parametrize("bug", ["roll direction", "swapped halves"])
+def test_cfg_ddim_bugs_are_caught(bug):
+    x, eps, _, coef = _ddim_setup()
+    exact = ct.cfg_ddim_ref(x, eps, coef, 9.0, 8)
+    if bug == "roll direction":
+        mutated, _ = ct.cfg_ddim_ref(x, eps, coef, 9.0, -8)
+    else:
+        mutated, _ = ct.cfg_ddim_ref(x, eps.flip(0), coef, 9.0, 8)
+    _caught(exact, mutated, torch.float32)
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_timestep_ref_matches_the_oracle_and_swapped_halves_are_caught(dtype):
+    from oracle.unet import Timesteps
+    t = torch.tensor([999.0, 1.0, 500.0, 21.0])
+    ref, bound = ct.timestep_ref(t, 320, dtype)
+    want = Timesteps(320)(t).double()  # fp32 frequencies and products: within the bound of the exact value
+    assert ((want - ref).abs() <= bound).all()
+    mutated = torch.cat([ref[:, 160:], ref[:, :160]], 1)
+    _caught((ref, bound), mutated, dtype)

@@ -1,7 +1,7 @@
-"""-m gpu: the bandwidth-bound kernels (GroupNorm stats / conv-prep / LayerNorm / conv_in / conv_out / CFG+DDIM /
-timestep embedding) against plain PyTorch fp32 on the same 16-bit-rounded inputs, and the EPPA tables against the
-oracle's get_masks / get_coords / SphericalPE (models/pano/utils.py:10-106, transformer.py:185-201)."""
-import math
+"""-m gpu: conv_in, the panorama branch's conv_out and copy2d against plain PyTorch fp32 on the same 16-bit-rounded
+inputs, pad_pano bit for bit, and the EPPA tables against the oracle's get_masks / get_coords / SphericalPE
+(models/pano/utils.py:10-106, transformer.py:185-201). GroupNorm, LayerNorm, CFG + DDIM and the timestep embedding are
+held to their fp64 contracts in test_gpu_norm_contract.py."""
 from types import SimpleNamespace
 
 import numpy as np
@@ -10,124 +10,6 @@ import torch
 import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
-
-
-def _tokens(x):  # NCHW -> [N*H*W, C]
-    n, c, h, w = x.shape
-    return x.permute(0, 2, 3, 1).reshape(n * h * w, c).contiguous()
-
-
-@pytest.mark.parametrize("N,C,H,W,circ", [(2, 320, 16, 32, 2), (3, 64, 8, 8, 0), (2, 1920, 8, 16, 2), (1, 640, 64, 128, 2),
-                                          (16, 320, 64, 64, 0)])
-def test_groupnorm_stats(cuda_device, N, C, H, W, circ):
-    from panfusion_b200 import ops
-    from oracle.eppa import pad_pano
-    x = (torch.randn(N, C, H, W, generator=torch.Generator().manual_seed(1)) * 1.7 + 0.3).bfloat16()
-    xp = pad_pano(x.float(), circ)
-    g = xp.reshape(N, 32, -1)
-    mean, var = g.mean(-1), g.var(-1, unbiased=False)
-    got = ops.groupnorm_stats(_tokens(x).to(cuda_device), N, H, W, 32, 1e-5, circ).cpu()
-    torch.testing.assert_close(got[..., 0], mean, rtol=1e-4, atol=1e-5)
-    torch.testing.assert_close(got[..., 1], (var + 1e-5).rsqrt(), rtol=1e-4, atol=1e-5)
-
-
-@pytest.mark.parametrize("circ,up,phases,halo", [(0, 1, 1, 1), (2, 1, 1, 1), (0, 1, 1, 0), (1, 2, 1, 1), (0, 2, 1, 1),
-                                                 (2, 1, 4, 1), (0, 1, 4, 1)])
-def test_conv_prep(cuda_device, circ, up, phases, halo):
-    """GroupNorm + SiLU + circular pad / upsample / zero halo / stride-2 phase split == the torch composition."""
-    from panfusion_b200 import ops
-    from oracle.eppa import pad_pano
-    N, C, H, W = 2, 128, 8, 12
-    g = torch.Generator().manual_seed(2)
-    x = torch.randn(N, C, H, W, generator=g).half()
-    gamma, beta = torch.randn(C, generator=g), torch.randn(C, generator=g)
-    xp = pad_pano(x.float(), circ)
-    ref = F.silu(F.group_norm(xp, 32, gamma, beta, 1e-5))  # stats over the padded tensor, like the reference
-    if up == 2:
-        ref = F.interpolate(ref, scale_factor=2.0, mode="nearest")
-    if halo:
-        ref = F.pad(ref, [1, 1, 1, 1])
-    if phases == 4:
-        ref = torch.stack([ref[:, :, py::2, px::2] for py in (0, 1) for px in (0, 1)], 0)  # [4,N,C,Ho+1,Wo+1]
-        ref = ref.permute(0, 1, 3, 4, 2)
-    else:
-        ref = ref.permute(0, 2, 3, 1)
-    xt = _tokens(x).to(cuda_device)
-    stats = ops.groupnorm_stats(xt, N, H, W, 32, 1e-5, circ)
-    got = ops.conv_prep(xt, N, H, W, stats=stats, gamma=gamma.to(cuda_device), beta=beta.to(cuda_device), groups=32,
-                        act=ops.PF_ACT_SILU, circ=circ, up=up, phases=phases, halo=halo)
-    torch.testing.assert_close(got.float().cpu().reshape(ref.shape), ref, rtol=2e-3, atol=2e-3)
-
-
-@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
-@pytest.mark.parametrize("N,C1,C2,H,W,circ_stats,circ,halo,act", [
-    (2, 128, 0, 8, 12, 0, 0, 1, "silu"),       # ResnetBlock2D norm1 / norm2, perspective branch
-    (2, 320, 0, 16, 32, 2, 2, 1, "silu"),      # panorama norm1: pad_pano(2) statistics and layout
-    (16, 320, 0, 64, 64, 0, 0, 1, "silu"),     # the level-0 shape of the benchmark (9 CTAs per image)
-    (3, 640, 0, 8, 8, 0, 0, 0, "none"),        # Transformer2DModel.norm: plain apply, no halo
-    (2, 320, 0, 8, 16, 0, 1, 1, "silu"),       # conv_norm_out: statistics of the un-padded tensor, pad_pano(1) layout
-    (2, 1280, 640, 8, 8, 0, 0, 1, "silu"),     # decoder: cat([hidden, skip]) with a group (60 ch) straddling the seam
-    (1, 640, 320, 16, 32, 2, 2, 1, "silu"),    # the same on the panorama branch
-    (20, 64, 64, 4, 4, 0, 0, 1, "silu"),       # many tiny images: one CTA per image
-])
-def test_gn_prep(cuda_device, dtype, N, C1, C2, H, W, circ_stats, circ, halo, act):
-    """pf_gn_prep (statistics + apply + layout + skip concatenation) against the torch composition pad_pano -> GroupNorm
-    -> SiLU -> pad of the reference (MVGenModel.py:110-115,223-231; diffusers ResnetBlock2D norm1/norm2) and against
-    pf_groupnorm_stats -> pf_conv_prep; the raw concatenation output is exact. Launched 3 times in a row with the same
-    bits each time: the per-image counters must re-arm themselves."""
-    from panfusion_b200 import ops
-    from oracle.eppa import pad_pano
-    g = torch.Generator().manual_seed(N + C1 + C2 + H)
-    C = C1 + C2
-    x = (torch.randn(N, C, H, W, generator=g) * 1.3 + 0.4).to(dtype)
-    gamma, beta = torch.randn(C, generator=g), torch.randn(C, generator=g)
-    xs = pad_pano(x.float(), circ_stats)
-    mean = xs.reshape(N, 32, -1).mean(-1)
-    var = xs.reshape(N, 32, -1).var(-1, unbiased=False)
-    cpg = C // 32
-    sc = (var + 1e-5).rsqrt().repeat_interleave(cpg, 1)[:, :, None, None] * gamma[None, :, None, None]
-    sh = beta[None, :, None, None] - mean.repeat_interleave(cpg, 1)[:, :, None, None] * sc
-    ref = pad_pano(x.float() * sc + sh, circ)
-    if act == "silu":
-        ref = F.silu(ref)
-    if halo:
-        ref = F.pad(ref, [1, 1, 1, 1])
-    ref = ref.permute(0, 2, 3, 1)
-    dev = cuda_device
-    xt = _tokens(x).to(dev)
-    x1, x2 = (xt[:, :C1].contiguous(), xt[:, C1:].contiguous()) if C2 else (xt, None)
-    kw = dict(gamma=gamma.to(dev), beta=beta.to(dev), groups=32, eps=1e-5,
-              act=ops.PF_ACT_SILU if act == "silu" else ops.PF_ACT_NONE, circ_stats=circ_stats, circ=circ, halo=halo)
-    outs = []
-    for _ in range(3):
-        r = ops.gn_prep(x1, N, H, W, x2=x2, want_cat=bool(C2), **kw)
-        got, cat = r if C2 else (r, None)
-        outs.append(got.clone())
-    torch.cuda.synchronize()
-    assert all(torch.equal(outs[0], o) for o in outs[1:])
-    if C2:
-        assert torch.equal(cat, xt)
-    tol = dict(rtol=2e-3, atol=2e-3) if dtype == torch.float16 else dict(rtol=1.6e-2, atol=1.6e-2)
-    torch.testing.assert_close(got.float().cpu().reshape(ref.shape), ref, **tol)
-    # the two-kernel path computes the same thing with a different partial-sum order: at most an output ulp apart
-    st = ops.groupnorm_stats(xt, N, H, W, 32, 1e-5, circ_stats)
-    two = ops.conv_prep(xt, N, H, W, stats=st, gamma=kw["gamma"], beta=kw["beta"], groups=32, act=kw["act"], circ=circ,
-                        halo=halo)
-    d = (got.float() - two.float()).abs()
-    assert (d > 0).float().mean().item() < 1e-3 and d.max().item() <= (2e-3 if dtype == torch.float16 else 3.2e-2) * max(1.0, two.float().abs().max().item())
-
-
-@pytest.mark.parametrize("T,C,with_pe", [(100, 320, True), (64, 1280, False), (33, 64, True), (256, 640, True)])
-def test_layernorm(cuda_device, T, C, with_pe):
-    from panfusion_b200 import ops
-    g = torch.Generator().manual_seed(3)
-    x = torch.randn(2 * T, C, generator=g).half()
-    gamma, beta = torch.randn(C, generator=g), torch.randn(C, generator=g)
-    pe = torch.randn(T, C, generator=g) if with_pe else None
-    ref = F.layer_norm(x.float() + (pe.repeat(2, 1) if with_pe else 0), (C,), gamma, beta, 1e-5)
-    got = ops.layernorm(x.to(cuda_device), gamma.to(cuda_device), beta.to(cuda_device), 1e-5,
-                        pe.to(cuda_device) if with_pe else None)
-    torch.testing.assert_close(got.float().cpu(), ref, rtol=1e-3, atol=2e-3)
 
 
 @pytest.mark.parametrize("circ", [False, True])
@@ -179,35 +61,12 @@ def test_conv_in_silu_layout_image(cuda_device, W):
     assert got[:, 16:].abs().max().item() == 0.0
 
 
-def test_timestep_embed_and_copy(cuda_device):
+def test_copy2d(cuda_device):
     from panfusion_b200 import ops
-    from oracle.unet import Timesteps
-    t = torch.tensor([981.0, 1.0, 500.0, 21.0])
-    ref = Timesteps(320)(t)
-    got = ops.timestep_embed(t.to(cuda_device), 320, torch.float16).float().cpu()
-    torch.testing.assert_close(got, ref, rtol=0, atol=2e-3)
     src = torch.randn(50, 64).half().to(cuda_device)
     dst = torch.zeros(50, 192, dtype=torch.float16, device=cuda_device)
     ops.copy2d(src, dst[:, 64:128])
     assert torch.equal(dst[:, 64:128], src) and dst[:, :64].abs().sum() == 0 and dst[:, 128:].abs().sum() == 0
-
-
-def test_cfg_ddim_step(cuda_device):
-    from panfusion_b200 import ops
-    from oracle.sampler import DDIM
-    g = torch.Generator().manual_seed(5)
-    x = torch.randn(1, 1, 4, 16, 32, generator=g)
-    eps = torch.randn(2, 1, 4, 16, 32, generator=g)
-    sched = DDIM()
-    sched.set_timesteps(50)
-    t = sched.timesteps[3]
-    e = eps[:1] + 9.0 * (eps[1:] - eps[:1])
-    ref = torch.roll(sched.step(e, t, x), 8, dims=-1)
-    a_t = sched.alphas_cumprod[int(t)].item()
-    a_p = sched.alphas_cumprod[int(t) - 20].item()
-    out = torch.empty_like(x, device=cuda_device)
-    ops.cfg_ddim_step(x.to(cuda_device), eps.to(cuda_device), out, 9.0, a_t, a_p, roll=8)
-    torch.testing.assert_close(out.cpu(), ref, rtol=1e-5, atol=1e-5)
 
 
 def _cams(n, seed=0):
