@@ -442,18 +442,24 @@ int pf_faedt_conv(const void* x, int B, int H, int W, int Cin, const void* w, co
  * dw [Cout][Cin_w][k][k] (torch layout) = f * sum_p x[p (+) tap, ci] dy[p, co], db [Cout] = f * sum_p dy[p, co] (db may be
  * NULL), f = inv_n / scale[0]. x fp16 [B, H, W, Cin] (Cin % 8 == 0, <= 128; channels >= Cin_w ignored), dy fp16
  * [B, Ho, Wo, Cdy] (Cdy % 8 == 0, <= 128; channels >= Cout ignored). ws: pf_faedt_wgrad_ws_floats(...) floats of fp32
- * per-chunk partials. Tensor-core split-K over pixel chunks, reduced in chunk order. */
+ * per-chunk partials. Tensor-core split-K over nch chunks of `chunk` pixels (a multiple of 32, at most ceil(P / 1024)
+ * chunks and 2^24 partial floats), reduced in chunk order. On return ws holds the unscaled partials
+ * [nch][k*k][Cin][Cdy] (sum over the chunk's pixels, all Cin x Cdy channels), then, when db is given, the chunk's dy
+ * column sums [nch][Cdy]. */
 long long pf_faedt_wgrad_ws_floats(int B, int Ho, int Wo, int Cin, int Cdy, int k);
 int pf_faedt_wgrad(const void* x, int B, int H, int W, int Cin, const void* dy, int Ho, int Wo, int Cdy, int Cin_w,
                    int Cout, int k, int stride, int pad, float* ws, const double* scale, double inv_n, float* dw,
                    float* db, int* flag, void* stream);
 /* BatchNorm2d in training mode (eps 1e-5) over z fp16 [P, C] (C 32/64/128, P > 1). ws: pf_faedt_bn_ws_floats(P, C).
- * pf_faedt_bn_stats: per-chunk Welford (count, mean, M2) merged in chunk order (Chan) -> stats fp32 [3][C] = batch
+ * Rows are reduced in nch chunks of max(256, ceil(P / 512)) rows; a chunk's channel c is split over 256 / C lanes.
+ * pf_faedt_bn_stats: per-chunk Welford (count, mean, M2), left in ws [nch][3][C], merged in chunk order (Chan) ->
+ * stats fp32 [3][C] = batch
  * mean, 1 / sqrt(biased var + eps), unbiased var; pending fp32 [2][C] <- (mean, unbiased var), which pf_faedt_adam folds
  * into the running statistics (momentum 0.1) only if the step is not skipped.
  * pf_faedt_bn_apply: out = relu?((z - mean) * invstd * gamma + beta) + residual? (fp16 [P, C]).
  * pf_faedt_bn_bwd: g' = g * (mask > 0) (mask = the ReLU output, or NULL), dz = gamma * invstd * (g' - mean g' -
- * xhat mean(g' xhat)) fp16; dgamma = f * sum g' xhat, dbeta = f * sum g' (fp32 [C], f = inv_n / scale[0]). */
+ * xhat mean(g' xhat)) fp16; dgamma = f * sum g' xhat, dbeta = f * sum g' (fp32 [C], f = inv_n / scale[0]). ws keeps
+ * the per-chunk (sum g', sum g' xhat) [nch][2][C] and, from float nch * 3 * C, (mean g', mean g' xhat) [2][C]. */
 long long pf_faedt_bn_ws_floats(long long P, int C);
 int pf_faedt_bn_stats(const void* z, long long P, int C, float* ws, float* stats, float* pending, void* stream);
 int pf_faedt_bn_apply(const void* z, long long P, int C, const float* stats, const float* gamma, const float* beta,

@@ -474,12 +474,12 @@ adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restric
   if (idx >= n) return;
   const double step = (double)(ictl[0] + 1);
   // torch's five fp32 kernels, each rounding once: Python's doubles cast to fp32 where torch passes them; division by
-  // the bias correction is a multiplication by its fp32 reciprocal, as torch's div by a CPU scalar is; lerp, addcmul
-  // and addcdiv compute self + w * (x) with one fused multiply-add. The intrinsics keep nvcc from contracting across
-  // what torch rounds separately.
+  // the bias correction is a multiplication by its reciprocal, taken in double and rounded to fp32 once, as torch's div
+  // by a CPU scalar is; lerp, addcmul and addcdiv compute self + w * (x) with one fused multiply-add. The intrinsics
+  // keep nvcc from contracting across what torch rounds separately.
   const double bc1 = 1.0 - pow(beta1, step), bc2 = 1.0 - pow(beta2, step);
   const float step_size = (float)(-(ctl[0] / bc1));
-  const float inv_bc2 = 1.f / (float)sqrt(bc2);
+  const float inv_bc2 = (float)(1.0 / sqrt(bc2));
   const float gv = g[idx];
   const float mv = __fmaf_rn((float)(1.0 - beta1), __fsub_rn(gv, m[idx]), m[idx]);
   const float vv = __fmaf_rn((float)(1.0 - beta2), __fmul_rn(gv, gv), __fmul_rn(v[idx], (float)beta2));

@@ -64,6 +64,56 @@ The normalisation and sampler kernels (csrc/norm.cu, csrc/elementwise.cu), u = 2
              logf (2u), two products (2u) and expf (4u) of ln f_i, then the product by t: |darg| <= u (4 |ln f_i| + 5)
              |t f_i|; cosf / sinf add 2 ulp of a value <= 1 (2^-22).
 
+The FAED training kernels (csrc/faed_train.cu), u = 2^-24, f = fl32(inv_n / S) (inv_n / S is exact in fp64: S is a
+power of two; the kernels round it to fp32 once):
+  wgrad part  (pf_faedt_wgrad's fp32 partial of one pixel chunk, in ws [nch][k^2][Cin][Cdy]) the chunk's
+             sum_p x[p (+) tap, ci] dy[p, co] on mma.sync m16n8k16 with an fp32 accumulator: fp16 x fp16 products are
+             exact in fp32, so only the accumulation rounds. One k-step adds 16 products to the accumulator; the tensor
+             core aligns them to the largest exponent and truncates, once when it sums the products and once when it
+             adds the accumulator, each time losing < 2^-23 of a magnitude <= the chunk's sum_p |x| |dy| so far.
+             Truncation errors all have the same sign, so they add linearly: |dpart| <= ceil(chunk / 16) 2^-22
+             sum_chunk |x| |dy|. (The convolution core's 2^-14 is the statistical sqrt(K) form; a partial sums one chunk
+             only, so the worst case stays small: 326 k-steps, 7.8e-5, at the largest chunk the models make, 5216 pixels
+             of the first layer at 4 x 512 x 1024.) The dY column sums for
+             db (ws [nch][Cdy] after the partials) are one thread's fp32 chain over the chunk: chunk u sum_chunk |dy|.
+  wgrad reduce  given the kernel's own partials, dw = fl(fl(sum_c part_c) f) summed in chunk order:
+             |dw - f sum_c part_c| <= nch u f sum_c |part_c| + u |dw|; db the same over the column sums.
+  wgrad      end to end against fp64 f sum_p x dy: the two bounds above with sum_c |part_c| <= sum |x| |dy|.
+  bn stats   (pf_faedt_bn_stats) chunks of row_chunk(P) rows, L = 256 / C lanes per channel, each lane a Welford
+             chain over n_w <= ceil(chunk / L) rows, then L - 1 Chan merges into lane 0, then nch Chan merges. The chunk
+             counts are exact integers. A Welford update rounds mu + d / k with error rho <= 3u A (A = max |z|: the
+             mean is large against the spread, so A, not the spread, sets the scale), and a rounding at update j moves
+             the lane mean by rho j / k afterwards: |dmean_lane| <= 3u A (n + 1) / 2. The same rounding moves M2 by
+             rho j (2 |mu_n - mu_j| + |mu_j - mu_{j-1}|) to first order (the later updates re-centre on the perturbed
+             mean); the products and sums add (n_w + 3) u M2. A Chan merge with delta = mean_b - mean_a and weight
+             w = n_a n_b / n_ab rounds the mean by 4u A and M2 by 2u (M2_a + M2_b + delta^2 w) + 4u delta^2 w, and
+             carries the means' errors into M2 as 2 |delta| w (dmean_a + dmean_b). The reference runs the kernel's
+             partition and merge order in fp64 and sums these terms. invstd = 1 / sqrt(M2 / n + eps): half the
+             relative error of M2 / n over var + eps, plus 4u (division, eps add, sqrtf, reciprocal); the unbiased
+             variance M2 / (n - 1) adds 2u. n is an fp32 count; past 2^24 it rounds by u. pending must be bit-equal
+             to stats rows 0 and 2.
+  bn apply   (pf_faedt_bn_apply) given the launch's fp32 stats: (z - mean), * invstd, * gamma, + beta each round once:
+             |dy| <= 3u |z - mean| invstd |gamma| + u |y|; ReLU is 1-Lipschitz; + residual rounds u |out|; fp16 store.
+  bn bwd     (pf_faedt_bn_bwd) g' = g (mask > 0) with the mask the STORED fp16 ReLU output, xhat = (z - mean) invstd from
+             the launch's fp32 stats (2u |xhat|). Per chunk (sum g', sum g' xhat) as the statistics' partition: n_w + L
+             additions, (n_w + L) u sum |g'| and (n_w + L + 3) u sum |g' xhat|; nch more additions merge them; sums =
+             the merged sums / P (one more u), dgamma = f sum g' xhat, dbeta = f sum g' (one more u). Given the launch's
+             sums, dz = gamma invstd (g' - s0 - xhat s1): 4u |gamma invstd| (|g'| + |s0| + 2 |xhat s1|) + fp16 store.
+  upsample   (pf_faedt_upsample) the weights are 0, 0.25, 0.75 or 1 and their products; w x is exact in fp32 and the two
+             lerps round <= 4 times: 4u (sum |w| |x|) + fp16 store. The backward gathers <= 4 x 4 outputs: <= 9 roundings
+             of the adjoint's magnitude, 10u (W^T |g|) + fp16 store.
+  loss       (pf_faedt_loss) pred = tanhf(o): <= 2 ulp of the fp64 tanh (2^-22 |pred| + 2^-149). loss = mean |pred - t|
+             over 3 B H W: a thread adds 3 ceil(M / 262144) terms (1024 x 256 threads grid-stride), an 8-level tree, the
+             final kernel adds 4 partials per thread and another 8-level tree: n = 3 ceil(M / 262144) + 20;
+             |dloss| <= (n u sum |d| + 2^-22 sum |pred| + u sum |d|) / count + u loss. seed = fl16(sign(d) (1 - pred^2) S)
+             with the kernel's pred: |seed - sign (1 - pred^2) S| <= 2^-11 |.| + 2u S + 2^-25 (fp32 products, the fp16
+             rounding); where |d| is within pred's error the sign is not defined and seed may be 0 or either sign,
+             except o = 0 against a zero target: tanhf(0) = 0 exactly, so d = 0 and sign(0) = 0 give a zero seed.
+             Channels 3..15 are exactly zero.
+  exact      pf_faedt_prep, pf_faedt_interleave and pf_faedt_pack (forward layout, stride-1 flipped kernel, the four
+             stride-2 phase kernels, zero padding) move or round values once: bit-equal.
+  adam       (pf_faedt_adam) torch.optim.Adam(foreach=False)'s five fp32 kernels, each rounding once: bit-equal.
+
 Every function here runs on whichever device its inputs live on (the CPU tests use the same code at small sizes).
 """
 from __future__ import annotations
@@ -516,3 +566,286 @@ def worst_ratio(got, ref, bound) -> float:
     assert stray == 0, f"{stray} elements written outside the contract's rows"
     r = ((got - ref).abs() / bound)[written]
     return float(torch.nan_to_num(r, nan=math.inf).max())
+
+
+# ---- FAED training (csrc/faed_train.cu) -----------------------------------------------------------------------------
+
+WGRAD_STAGE = 32  # pixels per wgrad pipeline stage
+WGRAD_KSTEP = 2.0 ** -22  # per mma k-step, of the chunk's sum |x| |dy|
+
+
+def faedt_factor(inv_n: float, scale: float) -> float:
+    """f = fl32(inv_n / S), the factor every parameter gradient is reduced with."""
+    return _f32(inv_n / scale)
+
+
+def wgrad_chunk(P: int, taps: int, Cin: int, Cdy: int) -> int:
+    """Pixels per wgrad chunk: at most 2^24 partial floats and at most ceil(P / 1024) chunks, a multiple of 32."""
+    cap = max(1, (1 << 24) // (taps * Cin * Cdy))
+    nch = min(-(-P // 1024), cap)
+    chunk = -(-P // nch)
+    return -(-chunk // WGRAD_STAGE) * WGRAD_STAGE
+
+
+def wgrad_ref(x, dy, *, Ho: int, Wo: int, k: int, stride: int, pad: int, chunk: int | None = None):
+    """pf_faedt_wgrad's partition of x fp16 [B, H, W, Cin] (rows outside [0, H) zero, columns circular) against dy fp16
+    [B, Ho, Wo, Cdy]: dict of fp64 `part` / `part_bound` [nch, k^2, Cin, Cdy], `dbpart` / `dbpart_bound` [nch, Cdy],
+    and the unscaled end-to-end sums `w` / `w_bound` [k^2, Cin, Cdy], `b` / `b_bound` [Cdy] (multiply by f)."""
+    B, H, W, Cin = x.shape
+    Cdy = dy.shape[-1]
+    P, taps = B * Ho * Wo, k * k
+    chunk = chunk or wgrad_chunk(P, taps, Cin, Cdy)
+    nch = -(-P // chunk)
+    dev = x.device
+    padrows = nch * chunk - P
+    d = torch.nn.functional.pad(dy.reshape(P, Cdy).double(), (0, 0, 0, padrows)).reshape(nch, chunk, Cdy)
+    da = d.abs()
+    p = torch.arange(P, device=dev)
+    b, oy, ox = p // (Ho * Wo), (p // Wo) % Ho, p % Wo
+    part = torch.empty((nch, taps, Cin, Cdy), dtype=torch.float64, device=dev)
+    mag = torch.empty_like(part)
+    for t in range(taps):
+        iy = oy * stride + t // k - pad
+        ix = (ox * stride + t % k - pad) % W
+        inside = ((iy >= 0) & (iy < H)).double()[:, None]
+        xt = x[b, iy.clamp(0, H - 1), ix].double() * inside
+        xt = torch.nn.functional.pad(xt, (0, 0, 0, padrows)).reshape(nch, chunk, Cin)
+        part[:, t] = xt.transpose(1, 2) @ d
+        mag[:, t] = xt.abs().transpose(1, 2) @ da
+        del xt
+    dbpart, dbmag = d.sum(1), da.sum(1)
+    steps = -(-chunk // 16)
+    return dict(part=part, part_bound=steps * WGRAD_KSTEP * mag + EXACT, dbpart=dbpart,
+                dbpart_bound=chunk * U * dbmag + EXACT, w=part.sum(0),
+                w_bound=(steps * WGRAD_KSTEP + nch * U) * mag.sum(0), b=dbpart.sum(0),
+                b_bound=(chunk + nch) * U * dbmag.sum(0), nch=nch, chunk=chunk)
+
+
+def wgrad_layout(t, Cin_w: int, Cout: int, k: int):
+    """[k^2, Cin, Cdy] -> dw's torch layout [Cout, Cin_w, k, k]."""
+    return t[:, :Cin_w, :Cout].permute(2, 1, 0).reshape(Cout, Cin_w, k, k)
+
+
+def wgrad_reduce_ref(part, f: float):
+    """(ref, bound) of f * sum_c part_c in chunk order, given the kernel's fp32 partials [nch, ...]."""
+    p = part.double()
+    ref = f * p.sum(0)
+    return ref, p.shape[0] * U * f * p.abs().sum(0) + U * ref.abs() + EXACT
+
+
+BN_EPS = 1e-5
+
+
+def bn_row_chunk(P: int) -> int:
+    """Rows per chunk of the BatchNorm reductions: at most 512 chunks, at least 256 rows each."""
+    return max(256, -(-P // 512))
+
+
+def _chan_merge(acc, b, A):
+    """Merge lane / chunk b into acc in fp64, carrying the error bounds of the kernel's fp32 Chan merge."""
+    n, mean, m2, em, e2 = acc
+    nb, mb, m2b, emb, e2b = b
+    nab = n + nb
+    live = nb > 0
+    delta = mb - mean
+    w = torch.where(live, n * nb / nab.clamp(min=1), torch.zeros_like(n))
+    q = delta * delta * w
+    e2n = e2 + e2b + 2 * delta.abs() * w * (em + emb) + 2 * U * (m2 + m2b + q) + 4 * U * q
+    emn = (n * em + nb * emb) / nab.clamp(min=1) + 4 * U * A
+    meann = mean + delta * nb / nab.clamp(min=1)
+    pick = lambda new, old: torch.where(live, new, old)
+    return (nab, pick(meann, mean), pick(m2 + m2b + q, m2), pick(emn, em), pick(e2n, e2))
+
+
+def bn_stats_ref(z, block: int = 64):
+    """pf_faedt_bn_stats of z fp16 [P, C]: dict of fp64 per-chunk `count` (exact), `mean` / `mean_bound`, `m2` /
+    `m2_bound` [nch, C], and the merged `stats` / `stats_bound` [3, C] (mean, invstd, unbiased var)."""
+    P, Cc = z.shape
+    L = 256 // Cc
+    chunk = bn_row_chunk(P)
+    nch = -(-P // chunk)
+    nw = -(-chunk // L)
+    dev = z.device
+    A = z.double().abs().amax(0)
+    outs = {key: [] for key in ("count", "mean", "m2", "em", "e2")}
+    for c0 in range(0, nch, block):
+        c1 = min(nch, c0 + block)
+        r0, r1 = c0 * chunk, min(P, c1 * chunk)
+        zz = torch.full(((c1 - c0) * chunk, Cc), float("nan"), dtype=torch.float64, device=dev)
+        zz[:r1 - r0] = z[r0:r1].double()
+        zz = torch.nn.functional.pad(zz.reshape(c1 - c0, chunk, Cc), (0, 0, 0, nw * L - chunk), value=float("nan"))
+        v = zz.reshape(c1 - c0, nw, L, Cc)                           # row t * L + lane of each chunk
+        valid = ~torch.isnan(v)
+        v0 = torch.where(valid, v, torch.zeros_like(v))
+        cnt = valid.double().cumsum(1)
+        mu = v0.cumsum(1) / cnt.clamp(min=1)                          # running means
+        n = cnt[:, -1]
+        mean = mu[:, -1]
+        m2 = (torch.where(valid, v0 - mean[:, None], torch.zeros_like(v0)) ** 2).sum(1)
+        prev = torch.cat([mu[:, :1], mu[:, :-1]], 1)
+        move = cnt * (2 * (mean[:, None] - mu).abs() + (mu - prev).abs())
+        e2 = 3 * U * A * torch.where(valid & (cnt >= 2), move, torch.zeros_like(move)).sum(1) + (nw + 3) * U * m2
+        em = 3 * U * A * (n + 1) / 2
+        acc = tuple(t[:, 0] for t in (n, mean, m2, em, e2))
+        for lane in range(1, L):
+            acc = _chan_merge(acc, tuple(t[:, lane] for t in (n, mean, m2, em, e2)), A)
+        for key, t in zip(outs, acc):
+            outs[key].append(t)
+        del zz, v, valid, v0, cnt, mu, prev, move
+    part = {key: torch.cat(t) for key, t in outs.items()}
+    zero = torch.zeros(Cc, dtype=torch.float64, device=dev)
+    acc = (zero, zero, zero, zero, zero)
+    for i in range(nch):
+        acc = _chan_merge(acc, tuple(part[key][i] for key in outs), A)
+    n, mean, m2, em, e2 = acc
+    eps = _f32(BN_EPS)
+    var = m2 / n
+    inv = 1.0 / torch.sqrt(var + eps)
+    nu = U if P > (1 << 24) else 0.0
+    stats = torch.stack([mean, inv, m2 / (n - 1)])
+    bound = torch.stack([em + EXACT, inv * (0.5 * (e2 / n + nu * var) / (var + eps) + 4 * U),
+                         e2 / (n - 1) + (2 * U + nu) * m2 / (n - 1)])
+    return dict(count=part["count"], mean=part["mean"], mean_bound=part["em"] + EXACT, m2=part["m2"],
+                m2_bound=part["e2"] + EXACT, stats=stats, stats_bound=bound, nch=nch, chunk=chunk)
+
+
+def bn_apply_ref(z, stats, gamma, beta, relu: bool, residual=None):
+    """(ref, bound) fp64 [P, C] of pf_faedt_bn_apply given the launch's fp32 stats [>= 2, C]."""
+    mean, inv = stats[0].double(), stats[1].double()
+    g, b = gamma.double(), beta.double()
+    c = z.double() - mean
+    y = c * inv * g + b
+    bound = 3 * U * c.abs() * inv * g.abs() + U * y.abs()
+    if relu:
+        y = y.clamp_min(0.0)
+    if residual is not None:
+        y = y + residual.double()
+        bound = bound + U * y.abs()
+    return y, bound + ulp_out(y, torch.float16)
+
+
+def bn_bwd_ref(g, mask, z, stats, gamma, f: float):
+    """pf_faedt_bn_bwd given the launch's fp32 stats: dict of fp64 per-chunk `part` / `part_bound` [nch, 2, C],
+    `sums` / `sums_bound` [2, C] and `dgamma`, `dbeta` (each with `_bound`), and dz_ref(sums) -> (ref, bound)."""
+    P, Cc = z.shape
+    L = 256 // Cc
+    chunk = bn_row_chunk(P)
+    nch = -(-P // chunk)
+    nw = -(-chunk // L)
+    gp = g.double()
+    if mask is not None:
+        gp = gp * (mask.double() > 0)
+    mean, inv = stats[0].double(), stats[1].double()
+    xh = (z.double() - mean) * inv
+    gx = gp * xh
+    pad = nch * chunk - P
+    cs = lambda t: torch.nn.functional.pad(t, (0, 0, 0, pad)).reshape(nch, chunk, Cc).sum(1)
+    s_g, s_gx, a_g, a_gx = cs(gp), cs(gx), cs(gp.abs()), cs(gx.abs())
+    part = torch.stack([s_g, s_gx], 1)
+    part_bound = torch.stack([(nw + L) * U * a_g, (nw + L + 3) * U * a_gx], 1) + EXACT
+    tot = part.sum(0)
+    tot_bound = part_bound.sum(0) + nch * U * torch.stack([a_g.sum(0), a_gx.sum(0)])
+    nu = U if P > (1 << 24) else 0.0
+    sums = tot / P
+    sums_bound = tot_bound / P + (U + nu) * sums.abs()
+    gam = gamma.double()
+
+    def dz_ref(sums_k):
+        s0, s1 = sums_k[0].double(), sums_k[1].double()
+        ref = gam * inv * (gp - s0 - xh * s1)
+        bound = 4 * U * (gam * inv).abs() * (gp.abs() + s0.abs() + 2 * (xh * s1).abs())
+        return ref, bound + ulp_out(ref, torch.float16)
+    return dict(part=part, part_bound=part_bound, sums=sums, sums_bound=sums_bound, dgamma=f * tot[1],
+                dgamma_bound=f * tot_bound[1] + U * f * tot[1].abs(), dbeta=f * tot[0],
+                dbeta_bound=f * tot_bound[0] + U * f * tot[0].abs(), dz_ref=dz_ref, nch=nch)
+
+
+def _up2(x):
+    return torch.nn.functional.interpolate(x, scale_factor=2, mode="bilinear", align_corners=False)
+
+
+def upsample_ref(x):
+    """(ref, bound) fp64 [B, 2H, 2W, C] of pf_faedt_upsample on x fp16 [B, H, W, C]."""
+    xd = x.double().permute(0, 3, 1, 2)
+    ref = _up2(xd).permute(0, 2, 3, 1)
+    mag = _up2(xd.abs()).permute(0, 2, 3, 1)
+    return ref, 4 * U * mag + ulp_out(ref, torch.float16)
+
+
+def upsample_bwd_ref(g, H: int, W: int):
+    """(ref, bound) fp64 [B, H, W, C] of pf_faedt_upsample_bwd: the adjoint of the bilinear x2 applied to g fp16
+    [B, 2H, 2W, C]."""
+    B, Cc = g.shape[0], g.shape[-1]
+    gd = g.double().permute(0, 3, 1, 2)
+    outs = []
+    for t in (gd, gd.abs()):
+        xr = torch.zeros((B, Cc, H, W), dtype=torch.float64, device=g.device, requires_grad=True)
+        with torch.enable_grad():
+            (gx,) = torch.autograd.grad(_up2(xr), xr, t)
+        outs.append(gx.permute(0, 2, 3, 1))
+    return outs[0], 10 * U * outs[1] + ulp_out(outs[0], torch.float16)
+
+
+def loss_ref(o, target, B: int, H: int, W: int):
+    """pf_faedt_loss: dict of fp64 `pred` / `pred_bound` [B, 3, H, W], `d` (tanh(o) - target) and `loss` /
+    `loss_bound`."""
+    pred = torch.tanh(o[..., :3].double()).permute(0, 3, 1, 2)
+    d = pred - (target.double() if target is not None else 0.0)
+    M = B * H * W
+    n = 3 * -(-M // (1024 * 256)) + 20
+    count = 3.0 * M
+    loss = d.abs().sum() / count
+    lb = ((n + 1) * U * d.abs().sum() + 2.0 ** -22 * pred.abs().sum()) / count + U * loss
+    return dict(pred=pred, pred_bound=2.0 ** -22 * pred.abs() + 2.0 ** -149, d=d, loss=loss, loss_bound=lb)
+
+
+def seed_check(seed, pred_k, d, pred_bound, S: float):
+    """(worst err/bound, number of elements whose sign is defined) of pf_faedt_loss's seed fp16 [B, H, W, 16] against
+    sign(d) (1 - pred^2) S computed from the kernel's fp32 pred [B, 3, H, W]; d = tanh(o) - target in fp64. Where
+    |d| <= pred's error the sign is not defined: there the seed must be 0 or either sign of the same magnitude.
+    Channels 3..15 must be exactly zero."""
+    assert not seed[..., 3:].any(), "seed channels 3..15 are not zero"
+    got = seed[..., :3].permute(0, 3, 1, 2).double()
+    p = pred_k.double()
+    mag = (1 - p * p) * S
+    bound = 2.0 ** -11 * mag.abs() + 2 * U * S + 2.0 ** -25
+    big = mag.abs() + bound >= 65520.0             # may round to inf in fp16
+    clear = d.abs() > pred_bound
+    want = torch.sign(d) * mag
+    err = torch.where(clear, (got - want).abs(), torch.minimum((got.abs() - mag).abs(), got.abs()))
+    r = err / bound
+    inf_ok = torch.isinf(got) & big & ((torch.sign(got) == torch.sign(d)) | ~clear)
+    r = torch.where(inf_ok, torch.zeros_like(r), r)
+    # tanhf(0) = 0 exactly: where the target is 0 too, d = 0 and sign(0) = 0 makes the seed exactly zero
+    r = torch.where((d == 0) & (p == 0) & (got != 0), torch.full_like(r, math.inf), r)
+    return float(torch.nan_to_num(r, nan=math.inf).max()), int(clear.sum())
+
+
+def prep_ref(src):
+    """pf_faedt_prep: fp32 [B, 3, H, W] -> fp16 [B, H, W, 16], channels 3..15 zero."""
+    out = torch.zeros(src.shape[0], src.shape[2], src.shape[3], 16, dtype=torch.float16, device=src.device)
+    out[..., :3] = src.permute(0, 2, 3, 1).half()
+    return out
+
+
+def interleave_ref(ph):
+    """pf_faedt_interleave: phases [4, B, H/2, W/2, C] -> [B, H, W, C], dx[b, 2q + r, 2p + c] = phases[2r + c]."""
+    _, B, h, w, Cc = ph.shape
+    return ph.reshape(2, 2, B, h, w, Cc).permute(2, 3, 0, 4, 1, 5).reshape(B, 2 * h, 2 * w, Cc)
+
+
+def pack_ref(w, k: int, stride: int, cin_pad: int, cw: int, dg_rows: int, dg_cw: int):
+    """pf_faedt_pack of w fp32 [Cout, Cin, k, k]: (fwd fp16 [k^2, cin_pad, cw], dg fp16) with zero padding; dg is the
+    flipped kernel [k^2, dg_rows, dg_cw] at stride 1 or the four phase kernels [4, 4, dg_rows, dg_cw] (phase (r, c)
+    tap (ty, tx) = w[.., 3 - 2 ty - r, 3 - 2 tx - c]) at stride 2."""
+    Cout, Cin = w.shape[:2]
+    fwd = torch.zeros(k * k, cin_pad, cw, dtype=torch.float32, device=w.device)
+    fwd[:, :Cin, :Cout] = w.permute(2, 3, 1, 0).reshape(k * k, Cin, Cout)
+    if stride == 1:
+        taps = w.flip(2, 3).permute(2, 3, 0, 1).reshape(k * k, Cout, Cin)
+    else:
+        taps = torch.cat([w[:, :, [3 - r, 1 - r]][:, :, :, [3 - c, 1 - c]].permute(2, 3, 0, 1).reshape(4, Cout, Cin)
+                          for r in (0, 1) for c in (0, 1)])
+    dg = torch.zeros(k * k, dg_rows, dg_cw, dtype=torch.float32, device=w.device)
+    dg[:, :Cout, :Cin] = taps
+    return fwd.half(), dg.half()

@@ -663,3 +663,358 @@ def test_timestep_ref_matches_the_oracle_and_swapped_halves_are_caught(dtype):
     assert ((want - ref).abs() <= bound).all()
     mutated = torch.cat([ref[:, 160:], ref[:, :160]], 1)
     _caught((ref, bound), mutated, dtype)
+
+
+# ---- FAED training kernels (faed_train.cu) --------------------------------------------------------------------------
+
+def _ratio(got, ref, bound):
+    return float(torch.nan_to_num((got.double() - ref).abs() / bound, nan=float("inf")).max())
+
+
+def _wgrad_setup(B=2, H=6, W=9, cin=16, cdy=16, k=3, s=1, seed=30):
+    g = torch.Generator().manual_seed(seed)
+    p = 1 if s == 2 else k // 2
+    Ho, Wo = (H + 2 * p - k) // s + 1, (W + 2 * p - k) // s + 1
+    x = torch.randn(B, H, W, cin, generator=g).half()
+    dy = torch.randn(B, Ho, Wo, cdy, generator=g).half()
+    return x, dy, dict(Ho=Ho, Wo=Wo, k=k, stride=s, pad=p)
+
+
+@pytest.mark.parametrize("k,s", [(3, 1), (9, 1), (4, 2)])
+def test_wgrad_ref_matches_autograd(k, s):
+    """wgrad_ref's dw / db (Cin_w < Cin, Cout < Cdy) equal autograd's weight gradient of conv2d on circular_pad."""
+    import torch.nn.functional as F
+    from panfusion_b200.faed_train import circular_pad
+    x, dy, kw = _wgrad_setup(W=12, k=k, s=s)
+    cin_w, cout = 3, 6
+    r = ct.wgrad_ref(x, dy, **kw)
+    w = torch.zeros(cout, cin_w, k, k, dtype=torch.float64, requires_grad=True)
+    b = torch.zeros(cout, dtype=torch.float64, requires_grad=True)
+    y = F.conv2d(circular_pad(x[..., :cin_w].permute(0, 3, 1, 2).double(), kw["pad"]), w, b, stride=s)
+    y.backward(dy[..., :cout].permute(0, 3, 1, 2).double())
+    assert torch.allclose(ct.wgrad_layout(r["w"], cin_w, cout, k), w.grad, rtol=1e-12, atol=1e-12)
+    assert torch.allclose(r["b"][:cout], b.grad, rtol=1e-12, atol=1e-12)
+    assert torch.allclose(r["part"].sum(0), r["w"]) and r["part"].shape[0] == r["nch"] > 1 or r["nch"] == 1
+
+
+def test_wgrad_chunk_restates_the_workspace_size():
+    """wgrad_chunk is the kernel's: 200 chunks of 1312 pixels for 32 -> 32 k9 at 256 x 1024 (the 2^24-float cap),
+    403 of 5216 for the first layer at 4 x 512 x 1024 (the largest chunk the trainer makes)."""
+    assert ct.wgrad_chunk(256 * 1024, 81, 32, 32) == 1312 and -(-256 * 1024 // 1312) == 200
+    assert ct.wgrad_chunk(4 * 512 * 1024, 81, 16, 32) == 5216 and -(-4 * 512 * 1024 // 5216) == 403
+    assert ct.wgrad_chunk(960, 9, 32, 32) == 960
+
+
+def _wgrad_bug(bug, chunk):
+    """(exact, mutated) partials / reduction / end-to-end for one emulated wgrad bug at the given chunk size."""
+    x, dy, kw = _wgrad_setup(B=1, H=2 * chunk // 32 if chunk > 1000 else 6, W=32 if chunk > 1000 else 9, cin=8, cdy=8,
+                             k=3, seed=31)
+    exact = ct.wgrad_ref(x, dy, chunk=chunk, **kw)
+    return x, dy, kw, exact
+
+
+@pytest.mark.parametrize("chunk", [64, 5216])
+@pytest.mark.parametrize("bug", ["seam read as zero", "last stage of a chunk dropped"])
+def test_wgrad_partial_bugs_are_caught(bug, chunk):
+    x, dy, kw, exact = _wgrad_bug(bug, chunk)
+    ok = _ratio(exact["part"].float(), exact["part"], exact["part_bound"])
+    if bug == "seam read as zero":
+        # taps kx = 0 read column W - 1 only through the wrap (ox = 0): zeroing it there is the bug
+        xo = x.clone()
+        xo[:, :, -1] = 0
+        mutated = exact["part"].clone()
+        mutated[:, 0::3] = ct.wgrad_ref(xo, dy, chunk=chunk, **kw)["part"][:, 0::3]
+    else:
+        dyd = dy.clone().reshape(-1, dy.shape[-1])
+        P = dyd.shape[0]
+        for c0 in range(0, P, chunk):
+            end = min(P, c0 + chunk)
+            last = (end - c0 - 1) // 32 * 32 + c0
+            dyd[last:end] = 0
+        mutated = ct.wgrad_ref(x, dyd.reshape(dy.shape), chunk=chunk, **kw)["part"]
+    bad = _ratio(mutated.float(), exact["part"], exact["part_bound"])
+    assert ok <= 1.0 < bad, (ok, bad)
+
+
+@pytest.mark.parametrize("bug", ["column sum added twice", "f applied as inv_n * S", "transposed tap"])
+def test_wgrad_reduction_bugs_are_caught(bug):
+    """The reduction of the kernel's partials (one chunk's dY column sum added twice, the factor inv_n * S) and the
+    end-to-end dw (dw[co][ci][kx][ky]); S = 2^10 with the trainer's inv_n of a 64 x 128 pair."""
+    x, dy, kw = _wgrad_setup(B=2, H=8, W=20, k=3, seed=32)
+    r = ct.wgrad_ref(x, dy, chunk=64, **kw)
+    inv_n, S = 1.0 / (3 * 2 * 64 * 128), 2.0 ** 10
+    f = ct.faedt_factor(inv_n, S)
+    part, dbpart = r["part"].float(), r["dbpart"].float()
+    ref, bound = ct.wgrad_reduce_ref(part, f)
+    dref, dbound = ct.wgrad_reduce_ref(dbpart, f)
+    good = (part.sum(0) * f, dbpart.sum(0) * f)
+    assert _ratio(good[0], ref, bound) <= 1.0 and _ratio(good[1], dref, dbound) <= 1.0
+    e2e_ok = _ratio(good[0], f * r["w"], f * r["w_bound"] + ct.U * f * r["w"].abs())
+    assert e2e_ok <= 1.0, e2e_ok
+    if bug == "column sum added twice":
+        bad = _ratio((dbpart.sum(0) + dbpart[1]) * f, dref, dbound)
+    elif bug == "f applied as inv_n * S":
+        bad = _ratio(part.sum(0) * ct._f32(inv_n * S), ref, bound)
+    else:
+        k = kw["k"]
+        t = part.sum(0) * f
+        tt = t.reshape(k, k, *t.shape[1:]).transpose(0, 1).reshape(t.shape)
+        bad = _ratio(tt, f * r["w"], f * r["w_bound"] + ct.U * f * r["w"].abs())
+    assert bad > 1.0, bad
+
+
+def _bn_operand(P, C, seed, mean=40.0, spread=0.5):
+    """A conv output before BN: each channel's bias (mean ~ 40) large against its spread."""
+    g = torch.Generator().manual_seed(seed)
+    return (mean + 5 * torch.randn(C, generator=g) + spread * torch.randn(P, C, generator=g)).half()
+
+
+@pytest.mark.parametrize("P,C", [(3007, 32), (257, 64), (16, 128)])
+def test_bn_refs_match_torch_batch_norm(P, C):
+    """bn_stats_ref / bn_apply_ref / bn_bwd_ref equal F.batch_norm(training=True), its running-statistic inputs and
+    its autograd (through ReLU, the mask from the output)."""
+    import torch.nn.functional as F
+    z = _bn_operand(P, C, seed=P + C)
+    g = torch.Generator().manual_seed(1)
+    gamma, beta = 0.5 + torch.rand(C, generator=g), 0.2 * torch.randn(C, generator=g)
+    st = ct.bn_stats_ref(z)
+    zd = z.double()
+    assert torch.equal(st["count"].sum(0), torch.full((C,), float(P), dtype=torch.float64))
+    assert torch.allclose(st["stats"][0], zd.mean(0), rtol=1e-12)
+    assert torch.allclose(st["stats"][1], 1 / torch.sqrt(zd.var(0, unbiased=False) + ct._f32(1e-5)), rtol=1e-10)
+    assert torch.allclose(st["stats"][2], zd.var(0, unbiased=True), rtol=1e-10)
+    assert (st["stats_bound"] > 0).all() and (st["m2_bound"] > 0).all()
+    stats = st["stats"]  # fp64 statistics: the references then equal torch's to fp64 rounding
+    zr = zd.clone().requires_grad_(True)
+    gr, br = gamma.double().requires_grad_(True), beta.double().requires_grad_(True)
+    out = F.batch_norm(zr, None, None, gr, br, True, 0.1, ct._f32(1e-5)).relu()
+    ref, _ = ct.bn_apply_ref(z, stats, gamma, beta, True)
+    assert torch.allclose(ref, out.detach(), rtol=1e-10, atol=1e-10)
+    gup = torch.randn(P, C, generator=g).half()
+    out.backward(gup.double())
+    bw = ct.bn_bwd_ref(gup, out.detach(), z, stats, gamma, 1.0)
+    assert torch.allclose(bw["dgamma"], gr.grad, rtol=1e-10, atol=1e-10)
+    assert torch.allclose(bw["dbeta"], br.grad, rtol=1e-12, atol=1e-12)
+    dz, _ = bw["dz_ref"](bw["sums"])
+    assert torch.allclose(dz, zr.grad, rtol=1e-8, atol=1e-8)
+
+
+def _bn_kernel_like_stats(z):
+    """Welford per lane, Chan merges, all in fp32: the kernel's own algorithm on the CPU (chunk counts as floats)."""
+    P, C = z.shape
+    L, chunk = 256 // C, ct.bn_row_chunk(z.shape[0])
+    zf = z.float()
+
+    def merge(a, b):
+        n, mean, m2 = a
+        nb, mb, m2b = b
+        live = nb > 0
+        nab = n + nb
+        delta = mb - mean
+        w = torch.where(live, nb / torch.where(live, nab, torch.ones_like(nab)), torch.zeros_like(nb))
+        mean2 = mean + delta * w
+        m22 = m2 + (m2b + delta * delta * (n * w))
+        return (torch.where(live, nab, n), torch.where(live, mean2, mean), torch.where(live, m22, m2))
+    parts, acc = [], None
+    for r0 in range(0, P, chunk):
+        lanes = []
+        for lane in range(L):
+            rows = zf[r0 + lane:min(P, r0 + chunk):L]
+            n, mean, m2 = torch.zeros(C), torch.zeros(C), torch.zeros(C)
+            for v in rows:
+                n = n + 1
+                d = v - mean
+                mean = mean + d / n
+                m2 = m2 + d * (v - mean)
+            lanes.append((n, mean, m2))
+        c = lanes[0]
+        for b in lanes[1:]:
+            c = merge(c, b)
+        parts.append(c)
+        acc = c if acc is None else merge(acc, c)
+    n, mean, m2 = acc
+    stats = torch.stack([mean, 1 / torch.sqrt(m2 / n + ct._f32(1e-5)), m2 / (n - 1)])
+    return parts, stats
+
+
+@pytest.mark.parametrize("P,C", [(257, 32), (600, 128)])
+def test_bn_stats_bound_accepts_fp32_welford(P, C):
+    """The kernel's algorithm run in fp32 on the CPU passes every per-chunk and merged bound; counts are exact."""
+    z = _bn_operand(P, C, seed=40)
+    st = ct.bn_stats_ref(z)
+    parts, stats = _bn_kernel_like_stats(z)
+    assert torch.equal(torch.stack([p[0] for p in parts]).double(), st["count"])
+    assert _ratio(torch.stack([p[1] for p in parts]), st["mean"], st["mean_bound"]) <= 1.0
+    assert _ratio(torch.stack([p[2] for p in parts]), st["m2"], st["m2_bound"]) <= 1.0
+    assert _ratio(stats, st["stats"], st["stats_bound"]) <= 1.0
+
+
+@pytest.mark.parametrize("P,C", [(257, 32), (16, 128)])
+def test_bn_stats_bugs_are_caught(P, C):
+    """A chunk's count off by one row (the last chunk of P = 257 has one); invstd from the unbiased variance."""
+    z = _bn_operand(P, C, seed=41)
+    st = ct.bn_stats_ref(z)
+    if P > 256:
+        short = ct.bn_stats_ref(z[:P - 1])
+        assert not torch.equal(short["count"].sum(0), st["count"].sum(0))
+    var_u = st["stats"][2]
+    mutated = st["stats"].clone()
+    mutated[1] = 1 / torch.sqrt(var_u + ct._f32(1e-5))
+    assert _ratio(st["stats"].float(), st["stats"], st["stats_bound"]) <= 1.0
+    assert _ratio(mutated.float(), st["stats"], st["stats_bound"]) > 1.0
+
+
+@pytest.mark.parametrize("bug", ["mask from pre-ReLU z", "dz without the xhat term"])
+def test_bn_bwd_bugs_are_caught(bug):
+    """At the trainer's deepest level (P = 16, C = 128) and at P = 3007, C = 32."""
+    for P, C in ((16, 128), (3007, 32)):
+        z = _bn_operand(P, C, seed=42, mean=0.3, spread=1.0)
+        g = torch.Generator().manual_seed(2)
+        gamma, beta = 0.5 + torch.rand(C, generator=g), 0.2 * torch.randn(C, generator=g)
+        stats = ct.bn_stats_ref(z)["stats"].float()
+        out = ct.bn_apply_ref(z, stats, gamma, beta, True)[0].half()
+        gup = torch.randn(P, C, generator=g).half()
+        bw = ct.bn_bwd_ref(gup, out, z, stats, gamma, 1.0)
+        ref, bound = bw["dz_ref"](bw["sums"].float())
+        assert _ratio(ref.half(), ref, bound) <= 1.0
+        if bug == "mask from pre-ReLU z":
+            mut = ct.bn_bwd_ref(gup, z, z, stats, gamma, 1.0)
+            bad = max(_ratio(mut["dbeta"].float(), bw["dbeta"], bw["dbeta_bound"]),
+                      _ratio(mut["dz_ref"](bw["sums"].float())[0].half(), ref, bound))
+        else:
+            s = bw["sums"].float().double()
+            bad = _ratio((gamma.double() * stats[1].double() * (gup.double() * (out.double() > 0) - s[0])).half(),
+                         ref, bound)
+        assert bad > 1.0, (P, C, bad)
+
+
+@pytest.mark.parametrize("H,W", [(1, 5), (5, 1), (3, 7), (4, 8)])
+def test_upsample_refs_match_interpolate_and_catch_bugs(H, W):
+    """upsample_ref is F.interpolate (bilinear, align_corners=False) and upsample_bwd_ref its autograd; align_corners
+    =True, a wrapped far edge and a backward gather missing output 2i - 1 are caught."""
+    import torch.nn.functional as F
+    g = torch.Generator().manual_seed(H * 10 + W)
+    x = torch.randn(2, H, W, 8, generator=g).half()
+    gy = torch.randn(2, 2 * H, 2 * W, 8, generator=g).half()
+    ref, bound = ct.upsample_ref(x)
+    xr = x.permute(0, 3, 1, 2).double().requires_grad_(True)
+    y = F.interpolate(xr, scale_factor=2, mode="bilinear", align_corners=False)
+    assert torch.allclose(ref, y.detach().permute(0, 2, 3, 1), rtol=1e-14, atol=1e-14)
+    y.backward(gy.permute(0, 3, 1, 2).double())
+    bref, bbound = ct.upsample_bwd_ref(gy, H, W)
+    assert torch.allclose(bref, xr.grad.permute(0, 2, 3, 1), rtol=1e-14, atol=1e-14)
+    assert _ratio(ref.half(), ref, bound) <= 1.0 and _ratio(bref.half(), bref, bbound) <= 1.0
+    xd = x.double().permute(0, 3, 1, 2)
+    bad = [_ratio(F.interpolate(xd, scale_factor=2, mode="bilinear", align_corners=True).permute(0, 2, 3, 1).half(),
+                  ref, bound)]
+    if W > 1:  # the far edge wrapped to column 0 instead of clamped
+        wrapped = F.interpolate(torch.cat([xd, xd[..., :1]], -1), size=(2 * H, 2 * W + 2), mode="bilinear",
+                                align_corners=False)
+        wrapped = F.interpolate(torch.cat([xd, xd[..., :1]], -1), scale_factor=2, mode="bilinear",
+                                align_corners=False)[..., :2 * W]
+        bad.append(_ratio(wrapped.permute(0, 2, 3, 1).half(), ref, bound))
+    # the gather over outputs 2i .. 2i + 2 only (output 2i - 1 dropped)
+    gd = gy.double().permute(0, 3, 1, 2)
+    miss = torch.zeros_like(gd)
+    miss[..., 0::2, :] = 1
+    miss[..., 0, :] = 1
+    keep_y = torch.ones(2 * H, dtype=torch.float64)
+    keep_y[1::2] = 0
+    keep_y[2 * H - 1] = 1 if H == 1 else 0
+    xr2 = torch.zeros_like(xr).requires_grad_(True)
+    yy = F.interpolate(xr2, scale_factor=2, mode="bilinear", align_corners=False)
+    # an input row iy keeps outputs 2 iy, 2 iy + 1, 2 iy + 2 and loses 2 iy - 1: emulate on a per-input basis
+    rows = []
+    for iy in range(H):
+        (gi,) = torch.autograd.grad(yy, xr2, gd * _drop_row_mask(H, W, iy), retain_graph=True)
+        rows.append(gi[..., iy, :])
+    missing = torch.stack(rows, -2).permute(0, 2, 3, 1)
+    if H > 1:
+        bad.append(_ratio(missing.half(), bref, bbound))
+    assert all(b > 1.0 for b in bad), bad
+
+
+def _drop_row_mask(H, W, iy):
+    """The outputs input row iy gathers from, without output row 2 iy - 1."""
+    m = torch.ones(2 * H, 2 * W, dtype=torch.float64)
+    if iy > 0:
+        m[2 * iy - 1] = 0
+    return m
+
+
+def _loss_setup(B=2, H=4, W=8, seed=50):
+    g = torch.Generator().manual_seed(seed)
+    o = torch.randn(B, H, W, 4, generator=g) * 2
+    t = torch.rand(B, 3, H, W, generator=g) * 2 - 1
+    o[0, 0, :3, :3] = 0
+    t[0, :, 0, :3] = 0  # d = 0 exactly: sign(0) = 0
+    return o, t
+
+
+def test_loss_ref_matches_torch_and_catches_bugs():
+    """pred = tanh, the L1 mean and autograd's seed direction; sign(0) = 1, a seed without (1 - pred^2) and the mean
+    over 4 channels are caught."""
+    B, H, W = 2, 4, 8
+    o, t = _loss_setup(B, H, W)
+    r = ct.loss_ref(o, t, B, H, W)
+    orr = o[..., :3].permute(0, 3, 1, 2).double().requires_grad_(True)
+    loss = (torch.tanh(orr) - t.double()).abs().mean()
+    loss.backward()
+    assert torch.allclose(r["loss"], loss.detach(), rtol=1e-14)
+    pred = r["pred"].float()
+    assert _ratio(pred, r["pred"], r["pred_bound"]) <= 1.0
+    S = 2.0 ** 15
+    # autograd's gradient is sign(d) (1 - tanh^2) / count: the seed is that times S * count
+    want = (orr.grad * 3 * B * H * W * S)
+    seed = torch.zeros(B, H, W, 16, dtype=torch.float16)
+    seed[..., :3] = want.permute(0, 2, 3, 1).half()
+    ok, n_clear = ct.seed_check(seed, pred, r["d"], r["pred_bound"], S)
+    assert ok <= 1.0 and n_clear > 0, ok
+    assert _ratio(torch.tensor(float(r["loss"])), r["loss"], r["loss_bound"]) <= 1.0
+    sign1 = torch.where(r["d"] == 0, torch.ones_like(r["d"]), torch.sign(r["d"]))
+    bad_seed = seed.clone()
+    bad_seed[..., :3] = (sign1 * (1 - pred.double() ** 2) * S).permute(0, 2, 3, 1).half()
+    assert ct.seed_check(bad_seed, pred, r["d"], r["pred_bound"], S)[0] > 1.0
+    bad_seed[..., :3] = (torch.sign(r["d"]) * S).permute(0, 2, 3, 1).half()
+    assert ct.seed_check(bad_seed, pred, r["d"], r["pred_bound"], S)[0] > 1.0
+    four = (r["d"].abs().sum() + (torch.tanh(o[..., 3].double())).abs().sum()) / (4 * B * H * W)
+    assert _ratio(four, r["loss"], r["loss_bound"]) > 1.0
+
+
+def test_pack_ref_adjoints_match_autograd():
+    """pack_ref's stride-1 flipped kernel and stride-2 phase kernels, convolved as FAEDTrainer._dgrad does, give
+    autograd's input gradient of the circular convolution (fp64, before the fp16 rounding)."""
+    import torch.nn.functional as F
+    from panfusion_b200.faed_train import circular_pad
+    g = torch.Generator().manual_seed(60)
+    for k, s in ((3, 1), (4, 2)):
+        cin, cout, B, H, W = 5, 6, 1, 6, 8
+        p = 1 if s == 2 else k // 2
+        w = torch.randn(cout, cin, k, k, generator=g, dtype=torch.float64)
+        x = torch.randn(B, cin, H, W, generator=g, dtype=torch.float64, requires_grad=True)
+        y = F.conv2d(circular_pad(x, p), w, stride=s)
+        gy = torch.randn(y.shape, generator=g, dtype=torch.float64)
+        y.backward(gy)
+        fwd, dg = pack_ref_fp64(w, k, s)
+        assert torch.equal(fwd[:, :cin, :cout], w.permute(2, 3, 1, 0).reshape(k * k, cin, cout))
+        if s == 1:
+            wt = dg.reshape(k, k, cout, cin).permute(3, 2, 0, 1)
+            dx = F.conv2d(circular_pad(gy, p), wt)
+        else:
+            dx = torch.zeros_like(x)
+            for r in (0, 1):
+                for c in (0, 1):
+                    wt = dg[4 * (2 * r + c):4 * (2 * r + c) + 4].reshape(2, 2, cout, cin).permute(3, 2, 0, 1)
+                    gp = F.pad(gy, (0, 0, 1 - r, r))
+                    gp = torch.cat([gp[..., gp.shape[-1] - (1 - c):], gp, gp[..., :c]], -1)
+                    dx[..., r::2, c::2] = F.conv2d(gp, wt)
+        assert torch.allclose(dx, x.grad, rtol=1e-12, atol=1e-12), (k, s)
+
+
+def pack_ref_fp64(w, k, s):
+    """pack_ref applied to the weights' flat indices (exact in fp16 below 2048), then to the fp64 weights."""
+    Cout, Cin = w.shape[:2]
+    idx = torch.arange(w.numel(), dtype=torch.float32).reshape(w.shape)
+    fi, di = ct.pack_ref(idx, k, s, Cin, Cout, Cout, Cin)
+    flat = w.reshape(-1)
+    return flat[fi.long()], flat[di.long()]

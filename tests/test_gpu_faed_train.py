@@ -108,7 +108,7 @@ def test_adam_matches_torch(cuda_device):
         ulp = (tr.params - ps.data).abs() / torch.finfo(torch.float32).eps / ref_mag
         diff = (tr.params != ps.data).sum().item()
         print(f"\nstep {step + 1}: {diff} of {ps.numel()} params differ, max {ulp.max().item():.2f} ulp")
-        assert ulp.max().item() <= 9.0  # measured 4.2 ulp on an H100; step 2 bit-equal
+        assert diff == 0, ulp.max().item()  # pf_faedt_adam rounds as torch's single-tensor Adam does
     st = opt.state[ps]
     assert torch.equal(tr.exp_avg, st["exp_avg"]) or (tr.exp_avg - st["exp_avg"]).abs().max() <= \
         1.2e-7 * st["exp_avg"].abs().max()
