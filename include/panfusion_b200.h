@@ -562,6 +562,22 @@ int pf_clip_score(const float* img_emb, const float* txt_emb, int B, int D, floa
                   void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * EvalPanoGen's crops and ground-truth resize (models/pano/EvalPanoGen.py:99-169, dataset/PanoDataset.py:140), uint8 in
+ * and out.
+ * pf_eval_crops: src uint8 [P, 3, H, W], cams N e2p camera records (PF_CAM_DOUBLES each, device) -> dst uint8
+ *   [N, 3, h, w]; crop n reads panorama n / crops_per_pano (N <= P * crops_per_pano, N <= 65535). Bilinear e2p with the
+ *   grid and taps of pf_e2p, accumulated as pf_e2p's fp32 path does, over texels t:
+ *     normalize = 1: t = float(x) / 255 (IEEE division), stored as uint8(trunc(v * 255)) -- the fp32 crop of
+ *                    `e2p(pano.float() / 255, ...)` as pf_inception_prep (normalize=True) and pf_clip_prep convert it;
+ *     normalize = 0: t = float(x), stored as uint8(trunc(v)) -- `e2p(pano.float(), ...).to(torch.uint8)`.
+ * pf_resize_area2_u8: src uint8 [B, C, H, W] -> dst uint8 [B, C, Ho, Wo] = cv2.resize(INTER_AREA) for H = 2 Ho and
+ *   W = 2 Wo: (a + b + c + d + 2) >> 2 per 2x2 block (OpenCV 4.x); Ho = H, Wo = W copies. Any other size is
+ *   PF_ERR_UNSUPPORTED (OpenCV rounds other integer factors half to even). */
+int pf_eval_crops(const uint8_t* src, int P, int H, int W, int crops_per_pano, int N, int h, int w, const double* cams,
+                  int normalize, uint8_t* dst, void* stream);
+int pf_resize_area2_u8(const uint8_t* src, int B, int C, int H, int W, int Ho, int Wo, uint8_t* dst, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * HorizonNet layout network (models/horizonnet/HorizonNet.py `net` = external/HorizonNet/model.py
  * HorizonNet('resnet50', use_rnn=True)). Activations are channels-last fp16 [B, H, W, C]; wrap_lr_pad's LR_PAD(p) +
  * Conv2d(padding=(p, 0)) (rows zero-padded, columns wrapped, corners zero) is addressing inside pf_hnet_conv. The LSTM's

@@ -96,6 +96,7 @@ EXPORTS = [
     "pf_inception_prep", "pf_conv2d_packed_cout", "pf_conv2d_nhwc", "pf_pool2d_nhwc", "pf_inception_head",
     "pf_inception_score_ws_doubles", "pf_inception_score",
     "pf_clip_prep_taps_ints", "pf_clip_prep_taps", "pf_clip_prep", "pf_clip_embed", "pf_clip_score",
+    "pf_eval_crops", "pf_resize_area2_u8",
     "pf_hnet_prep", "pf_hnet_conv", "pf_hnet_height_upsample", "pf_lstm_bidir", "pf_lstm_bidir_clusters",
     "pf_hnet_head", "pf_layout_render", "pf_layout_condition",
 ]

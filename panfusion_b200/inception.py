@@ -286,6 +286,15 @@ def _check_images(net: InceptionV3, imgs: torch.Tensor, normalize: bool) -> None
                          "move the metric with .to(device)")
 
 
+def _check_features(f: torch.Tensor, width: int, device: torch.device) -> None:
+    _lib.require_cuda(f)
+    if f.dtype != torch.float32 or f.dim() != 2 or f.shape[1] != width:
+        raise ValueError(f"expected fp32 features [n, {width}], got {f.dtype} {tuple(f.shape)}")
+    if f.device != device:
+        raise ValueError(f"features are on {f.device} but the metric's states on {device}; "
+                         "move the metric with .to(device)")
+
+
 class FrechetInceptionDistance(nn.Module):
     """torchmetrics' FrechetInceptionDistance(feature=2048) on the GPU: update(imgs, real), compute() -> 0-d fp32 CUDA
     tensor, reset(). `inception=` shares one packed network between metric objects."""
@@ -322,13 +331,21 @@ class FrechetInceptionDistance(nn.Module):
             raise ValueError(f"images are on {imgs.device} but the metric's states on "
                              f"{self.real_features_sum.device}; move the metric with .to(device)")
         feats, _ = self.inception(imgs, normalize=self.normalize)
+        self.update_features(feats, real)
+
+    @torch.no_grad()
+    def update_features(self, pool3: torch.Tensor, real: bool) -> None:
+        """update() from pool3 features [n, 2048] fp32 (CUDA) that the caller took from this metric's network, so one
+        forward can feed several metrics."""
+        _check_features(pool3, FEATURES, self.real_features_sum.device)
+        pool3 = pool3.contiguous()
         side = "real" if real else "fake"
         s, c = getattr(self, f"{side}_features_sum"), getattr(self, f"{side}_features_cov_sum")
-        with torch.cuda.device(imgs.device):
-            _lib.check(_lib.lib().pf_faed_stats(C.c_void_p(feats.data_ptr()), feats.shape[0], FEATURES,
+        with torch.cuda.device(pool3.device):
+            _lib.check(_lib.lib().pf_faed_stats(C.c_void_p(pool3.data_ptr()), pool3.shape[0], FEATURES,
                                                 C.c_void_p(s.data_ptr()), C.c_void_p(c.data_ptr()),
                                                 C.c_void_p(_lib.stream_ptr())))
-        getattr(self, f"{side}_features_num_samples").add_(imgs.shape[0])
+        getattr(self, f"{side}_features_num_samples").add_(pool3.shape[0])
         self._update_called = True
 
     def compute(self) -> torch.Tensor:
@@ -369,7 +386,14 @@ class InceptionScore(nn.Module):
     @torch.no_grad()
     def update(self, imgs: torch.Tensor) -> None:
         _check_images(self.inception, imgs, self.normalize)
-        self.features.append(self.inception(imgs, normalize=self.normalize)[1])
+        self.update_logits(self.inception(imgs, normalize=self.normalize)[1])
+
+    @torch.no_grad()
+    def update_logits(self, logits: torch.Tensor) -> None:
+        """update() from logits_unbiased [n, 1008] fp32 (CUDA) that the caller took from this metric's network. Rows
+        are kept in call order, which compute()'s randperm indexes."""
+        _check_features(logits, CLASSES, self.inception.fc_w.device)
+        self.features.append(logits)
         self._update_called = True
 
     def compute(self) -> tuple[torch.Tensor, torch.Tensor]:
