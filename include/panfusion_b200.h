@@ -293,7 +293,7 @@ int pf_pad_pano(const void* x, void* out, int elem_bytes, long long rows, int W,
 /* out[r, :cols] = softmax(scale * s[r, :cols]) — fp32 logits [rows, ld] -> 16-bit probabilities [rows, ldo].
  * The VAE mid-block attention (diffusers AutoencoderKL [3P], called through decode_latent, PanoGenerator.py:272-278)
  * has ONE head of width 512, outside the flash kernel's head sizes: it runs as pf_gemm_taps (Q K^T, fp32 out) ->
- * pf_softmax_rows -> pf_gemm_taps (P V). */
+ * pf_softmax_rows -> pf_gemm_taps (P V). out must be 4-byte aligned and ldo even (column pairs are stored as words). */
 int pf_softmax_rows(const float* s, long long ld, void* out, long long ldo, int dtype, long long rows, int cols,
                     float scale, void* stream);
 
@@ -324,7 +324,7 @@ int pf_embed_tokens(const long long* ids, const float* tok_emb, const float* pos
 /* Latent sampling at the end of the VAE encoder (diffusers DiagonalGaussianDistribution.sample [3P] + the scaling of
  * PanoGenerator.encode_image, models/pano/PanoGenerator.py:218-224): moments = channels-last rows of width ld holding
  * [mean (L) | logvar (L) | ...] for N images of HW pixels; eps, out NCHW fp32 [N, L, HW];
- * out = (mean + exp(0.5 * clamp(logvar, -30, 20)) * eps) * scale. */
+ * out = (mean + exp(0.5 * clamp(logvar, -30, 20)) * eps) * scale; like torch.clamp, the clamp keeps a NaN logvar NaN. */
 int pf_gaussian_sample(const float* moments, int ld, const float* eps, float* out, int N, int L, int HW, float scale,
                        void* stream);
 int pf_add_noise(const float* x0, const float* noise, float* out, const long long* t, const float* alphas_cumprod,

@@ -316,7 +316,9 @@ gaussian_sample_kernel(const float* __restrict__ moments, int ld, const float* _
   const long long n = r / L;
   const float* row = moments + (n * HW + px) * (long long)ld;
   const float mean = __ldg(row + c);
-  const float logvar = fminf(fmaxf(__ldg(row + L + c), -30.0f), 20.0f);
+  // torch.clamp propagates NaN; fmaxf / fminf would turn a NaN logvar into -30 and hide a diverged encoder
+  const float lv = __ldg(row + L + c);
+  const float logvar = isnan(lv) ? lv : fminf(fmaxf(lv, -30.0f), 20.0f);
   const float stdv = expf(__fmul_rn(0.5f, logvar));
   out[idx] = __fmul_rn(__fadd_rn(mean, __fmul_rn(stdv, __ldg(eps + idx))), scale);
 }
@@ -390,6 +392,8 @@ extern "C" int pf_softmax_rows(const float* s, long long ld, void* out, long lon
   PF_CHECK_ARG(dtype == PF_BF16 || dtype == PF_F16, "pf_softmax_rows: 16-bit output dtype required");
   PF_CHECK_ARG(rows > 0 && rows <= 2147483647LL && cols > 0 && ld >= cols && ldo >= cols && ldo % 2 == 0,
                "pf_softmax_rows: bad shape rows=%lld cols=%d", rows, cols);
+  // the kernel stores column pairs as 32-bit words: every output row must start 4-byte aligned
+  PF_CHECK_ARG(((uintptr_t)out & 3) == 0, "pf_softmax_rows: out must be 4-byte aligned");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (dtype == PF_BF16) softmax_rows_kernel<true><<<(unsigned)rows, 256, 0, st>>>(s, ld, static_cast<uint16_t*>(out), ldo, cols, scale);
   else softmax_rows_kernel<false><<<(unsigned)rows, 256, 0, st>>>(s, ld, static_cast<uint16_t*>(out), ldo, cols, scale);

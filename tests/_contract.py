@@ -64,6 +64,29 @@ The normalisation and sampler kernels (csrc/norm.cu, csrc/elementwise.cu), u = 2
              logf (2u), two products (2u) and expf (4u) of ln f_i, then the product by t: |darg| <= u (4 |ln f_i| + 5)
              |t f_i|; cosf / sinf add 2 ulp of a value <= 1 (2^-22).
 
+The remaining element-wise kernels of csrc/elementwise.cu, u = 2^-24:
+  conv_in    (pf_conv_in) 3 x 3, pad 1 convolution of fp32 NCHW x with fp32 weights: rows zero-padded, columns
+             zero-padded or wrapped (circ). A thread seeds its fp32 accumulator with the bias and adds the K = 9 Cin taps
+             by fmaf, one rounding each, so the sequential-FMA bound holds: |dacc| <= gamma_K (|b| + sum |x| |w|),
+             gamma_K = K u / (1 - K u). SiLU adds what it adds in gn apply (1.13 |dacc| + 2^-20 (1 + |y|) |silu(y)|),
+             then the 16-bit store one output ulp. An element whose terms and bias are all zero (the zero-padded output
+             channels) must be exactly zero.
+  softmax    (pf_softmax_rows) p_j = e_j / sum e, e_j = expf(fl(fl(x_j - m) scale)), m the row's unscaled maximum (exact).
+             The argument carries two roundings, an absolute error of 2u |a_j| (a_j = (x_j - m) scale <= 0), which moves
+             e_j by a relative 2u |a_j|: large only where e_j = e^{a_j} is tiny. expf adds 2 ulp (4u; build.py uses
+             no fast-math). The denominator adds positive terms: a thread adds ceil(cols / 256) of them, then a 5-level
+             shuffle tree and the 8 warp partials in series, so dS <= sum_j e_j (2u |a_j| + 4u) + n_S u S with
+             n_S = ceil(cols / 256) + 13. The reciprocal and the product round once each: |dp_j| <= p_j (2u |a_j| + 4u +
+             dS / S + 2u), then the 16-bit store.
+  gaussian   (pf_gaussian_sample) z = (mean + exp(0.5 clamp(logvar, -30, 20)) eps) scale; 0.5 lv is exact, expf 4u, the
+             product, the sum and the scale one rounding each: |dz| <= |scale| (5u |t| + u |mean + t|) + u |z|,
+             t = std eps. The clamp propagates NaN like torch.clamp: a NaN mean or logvar gives a NaN z.
+  mse        (pf_mse_loss) sum (a - b)^2 / n over a fixed partition of 296 chunks of ceil(n / 296) elements. d = a - b
+             rounds (2u of d^2), a thread's fmaf chain adds ceil(chunk / 256) terms, a 5-level shuffle tree and the 8
+             warp partials in series follow, all on non-negative values: n_M = ceil(chunk / 256) + 14 and each chunk's
+             fp32 sum errs by <= n_M u of its sum. The 296 partials are added and divided by n in fp64 (2^-50, under the
+             slack), then rounded to fp32: |dloss| <= n_M u sum d^2 / n + u loss.
+
 The FAED training kernels (csrc/faed_train.cu), u = 2^-24, f = fl32(inv_n / S) (inv_n / S is exact in fp64: S is a
 power of two; the kernels round it to fp32 once):
   wgrad part  (pf_faedt_wgrad's fp32 partial of one pixel chunk, in ws [nch][k^2][Cin][Cdy]) the chunk's
@@ -555,6 +578,74 @@ def timestep_ref(t, dim: int, out_dtype: torch.dtype):
     ref = torch.cat([arg.cos(), arg.sin()], 1)
     b = U * (4 * lnf.abs() + 5) * arg.abs() + 2.0 ** -22
     return ref, torch.cat([b, b], 1) + ulp_out(ref, out_dtype)
+
+
+def conv_in_ref(x, w, b, circ: bool, act: int, out_dtype: torch.dtype):
+    """(ref, bound), fp64 tokens [N * H * W, Cout]: pf_conv_in of the fp32 NCHW x [N, Cin, H, W] the kernel reads with
+    fp32 weights w [Cout, Cin, 3, 3] and bias b [Cout] (None: no bias)."""
+    W = x.shape[-1]
+    xd = x.double()
+    xd = xd[..., torch.arange(-1, W + 1, device=x.device) % W] if circ else torch.nn.functional.pad(xd, (1, 1))
+    xd = torch.nn.functional.pad(xd, (0, 0, 1, 1))
+    wd = w.double()
+    acc = torch.nn.functional.conv2d(xd, wd)
+    mag = torch.nn.functional.conv2d(xd.abs(), wd.abs())
+    if b is not None:
+        acc += b.double()[:, None, None]
+        mag += b.double().abs()[:, None, None]
+    K = w.shape[1] * 9
+    err = K * U / (1 - K * U) * mag
+    if act == ACT_SILU:
+        s = _silu(acc)
+        err = ACT_LIP * err + SILU_REL * (1.0 + acc.abs()) * s.abs()
+        acc = s
+    tok = lambda t: t.permute(0, 2, 3, 1).reshape(-1, t.shape[1])
+    ref, mag = tok(acc), tok(mag)
+    bound = tok(err) + ulp_out(ref, out_dtype)
+    return ref, torch.where(mag == 0, torch.full_like(bound, EXACT), bound)
+
+
+def softmax_rows_ref(s, scale: float, out_dtype: torch.dtype):
+    """(ref, bound), fp64 [rows, cols]: pf_softmax_rows of the fp32 logits s [rows, cols] (any row stride) at the fp32
+    value of `scale`."""
+    scale = _f32(scale)
+    x = s.double()
+    a = (x - x.amax(1, keepdim=True)) * scale
+    e = torch.exp(a)
+    S = e.sum(1, keepdim=True)
+    n_s = -(-s.shape[1] // 256) + 13
+    rel_e = 2 * U * a.abs() + 4 * U
+    dS = (e * rel_e).sum(1, keepdim=True) + n_s * U * S
+    p = e / S
+    return p, p * (rel_e + dS / S + 2 * U) + ulp_out(p, out_dtype)
+
+
+def gaussian_sample_ref(moments, ld: int, eps, L: int, scale: float):
+    """(ref, bound), fp64 NCHW like eps [N, L, h, w]: pf_gaussian_sample of the channels-last fp32 moments rows of
+    width ld ([mean (L) | logvar (L) | ...], N * h * w rows from moments' first element). NaN where mean or logvar is
+    NaN (ref and bound)."""
+    N, _, h, w = eps.shape
+    rows = moments.as_strided((N * h * w, 2 * L), (ld, 1))
+    m4 = rows.double().reshape(N, h, w, 2 * L).permute(0, 3, 1, 2)
+    mean, logvar = m4[:, :L], m4[:, L:].clamp(-30.0, 20.0)
+    scale = _f32(scale)
+    t = torch.exp(0.5 * logvar) * eps.double()
+    ref = (mean + t) * scale
+    bound = abs(scale) * (5 * U * t.abs() + U * (mean + t).abs()) + U * ref.abs() + EXACT
+    return ref, bound
+
+
+MSE_CTAS = 296  # elementwise.cu: the fixed partition of pf_mse_loss
+
+
+def mse_ref(a, b):
+    """(ref, bound), fp64 scalars: pf_mse_loss of the fp32 a, b (any shape, n elements)."""
+    n = a.numel()
+    d2 = (a.double() - b.double()).reshape(-1) ** 2
+    chunk = -(-n // MSE_CTAS)
+    n_m = -(-chunk // 256) + 14
+    ref = d2.sum() / n
+    return ref, n_m * U * ref + U * ref + EXACT
 
 
 def worst_ratio(got, ref, bound) -> float:

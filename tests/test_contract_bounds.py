@@ -10,7 +10,12 @@ previous image, a store past Cout and a shifted output slice. The normalisation 
 LayerNorm, the token embedding's row statistics, CFG + DDIM, the timestep embedding) are pinned to F.group_norm on
 pad_pano, F.layer_norm, the oracle's DDIM step and Timesteps, then shown to catch a dropped pixel, a one-sided seam
 weight, a count over the unpadded width, the next group's or another image's statistics, a block-indexed PE, a skipped
-token, a reversed roll, swapped CFG halves, swapped sin / cos halves and statistics of the unrounded row."""
+token, a reversed roll, swapped CFG halves, swapped sin / cos halves and statistics of the unrounded row. The conv_in,
+VAE softmax, latent sampling and MSE references are pinned to F.conv2d (on pad_pano for the circular case),
+torch.softmax, the DiagonalGaussianDistribution.sample formula and F.mse_loss, then shown to catch a seam wrapped to
+zero, a tap reading the previous image, a missing bias, SiLU before the bias, the decoder fold's ones channel padded
+with ones, logits scaled before the maximum is subtracted, a dropped last odd column, a clamp at 30, swapped mean and
+logvar, an NHWC output and a mean over the padded element count."""
 import pytest
 import torch
 
@@ -1018,3 +1023,185 @@ def pack_ref_fp64(w, k, s):
     fi, di = ct.pack_ref(idx, k, s, Cin, Cout, Cout, Cin)
     flat = w.reshape(-1)
     return flat[fi.long()], flat[di.long()]
+
+
+# ---- conv_in, VAE softmax, latent sampling, training loss (elementwise.cu) ------------------------------------------
+
+def _conv_in_setup(N=2, Cin=4, H=5, W=8, Cout=16, seed=70):
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(N, Cin, H, W, generator=g)
+    x[..., 0] += 2.0   # the seam columns differ from their wrapped neighbours
+    x[..., -1] -= 2.0
+    w = torch.randn(Cout, Cin, 3, 3, generator=g) * 0.3
+    return g, x, w, torch.randn(Cout, generator=g)
+
+
+def _tokens(t):
+    return t.double().permute(0, 2, 3, 1).reshape(-1, t.shape[1])
+
+
+@pytest.mark.parametrize("circ", [False, True])
+@pytest.mark.parametrize("act", [ct.ACT_NONE, ct.ACT_SILU])
+def test_conv_in_ref_matches_torch(circ, act):
+    """conv_in_ref equals F.conv2d (on pad_pano(x, 1) for the circular case, rows zero-padded), then SiLU."""
+    import torch.nn.functional as F
+    from oracle.eppa import pad_pano, unpad_pano
+    _, x, w, b = _conv_in_setup()
+    xd, wd, bd = x.double(), w.double(), b.double()
+    want = unpad_pano(F.conv2d(pad_pano(xd, 1), wd, bd, padding=1), 1) if circ else F.conv2d(xd, wd, bd, padding=1)
+    if act == ct.ACT_SILU:
+        want = F.silu(want)
+    ref, bound = ct.conv_in_ref(x, w, b, circ, act, torch.float16)
+    assert torch.allclose(ref, _tokens(want), rtol=1e-12, atol=1e-12) and (bound > 0).all()
+
+
+def test_conv_in_ref_of_the_decoder_fold_matches_post_quant_then_conv_in():
+    """VAEDecoderPack's fold: conv_in over [z | ones] with the composed weights equals post_quant_conv (1 x 1) followed
+    by conv_in with zero padding; zero output channels (the ControlNet's padding to 64) must be exact zeros."""
+    import torch.nn.functional as F
+    g, z, wi, b = _conv_in_setup(Cin=4, Cout=16, seed=71)
+    wq, bq = torch.randn(4, 4, generator=g).double(), torch.randn(4, generator=g).double()
+    w5 = torch.cat([torch.einsum("octs,ci->oits", wi.double(), wq), torch.einsum("octs,c->ots", wi.double(), bq)[:, None]], 1)
+    x5 = torch.cat([z, torch.ones_like(z[:, :1])], 1)
+    ref, _ = ct.conv_in_ref(x5, w5, b, False, ct.ACT_NONE, torch.float16)
+    want = F.conv2d(F.conv2d(z.double(), wq[..., None, None], bq), wi.double(), b.double(), padding=1)
+    assert torch.allclose(ref, _tokens(want), rtol=1e-12, atol=1e-12)
+    wp, bp = torch.zeros(64, 4, 3, 3), torch.zeros(64)
+    wp[:16], bp[:16] = wi, b
+    _, bound = ct.conv_in_ref(z, wp, bp, False, ct.ACT_SILU, torch.float16)
+    assert (bound[:, 16:] == ct.EXACT).all() and (bound[:, :16] > ct.EXACT).all()
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+@pytest.mark.parametrize("bug", ["seam wrapped to zero", "previous image's last row", "missing bias",
+                                 "silu before the bias", "ones channel padded as data"])
+def test_conv_in_bugs_are_caught(dtype, bug):
+    """The seam column read as zero padding; row 0 of image n reading image n - 1's last row (the images stacked
+    without a border); the bias never seeded; SiLU applied before the bias; the decoder fold's ones channel padded
+    with ones (post_quant_conv's bias folded into conv_in's bias), which changes only the border pixels."""
+    g, x, w, b = _conv_in_setup(Cin=5 if bug == "ones channel padded as data" else 4)
+    circ = bug == "seam wrapped to zero"
+    act = ct.ACT_SILU if bug == "silu before the bias" else ct.ACT_NONE
+    if bug == "ones channel padded as data":
+        x[:, 4] = 1.0
+    exact = ct.conv_in_ref(x, w, b, circ, act, dtype)
+    N, Cin, H, W = x.shape
+    if bug == "seam wrapped to zero":
+        mutated, _ = ct.conv_in_ref(x, w, b, False, act, dtype)
+    elif bug == "previous image's last row":
+        stacked = x.permute(1, 0, 2, 3).reshape(1, Cin, N * H, W)
+        mutated, _ = ct.conv_in_ref(stacked, w, b, circ, act, dtype)
+    elif bug == "missing bias":
+        mutated, _ = ct.conv_in_ref(x, w, None, circ, act, dtype)
+    elif bug == "silu before the bias":
+        mutated = ct.conv_in_ref(x, w, None, circ, act, dtype)[0] + b.double()
+    else:
+        mutated, _ = ct.conv_in_ref(x[:, :4], w[:, :4], b + w[:, 4].sum((1, 2)), circ, act, dtype)
+    _caught(exact, mutated, dtype)
+
+
+def _softmax_logits(rows, cols, scale, seed=72):
+    """Logits as the VAE attention makes them: each row its own offset, a spread of +-50 after scaling."""
+    g = torch.Generator().manual_seed(seed)
+    off = 400 * torch.rand(rows, 1, generator=g) - 200
+    return (off + 50 * (2 * torch.rand(rows, cols, generator=g) - 1)) / scale
+
+
+def test_softmax_rows_ref_matches_torch_softmax():
+    scale = 512 ** -0.5
+    s = _softmax_logits(6, 777, scale)
+    ref, bound = ct.softmax_rows_ref(s[:, :700], scale, torch.float16)  # a view with ld > cols
+    want = torch.softmax(ct._f32(scale) * s[:, :700].double(), -1)
+    assert torch.allclose(ref, want, rtol=1e-12, atol=0) and (bound > 0).all()
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+@pytest.mark.parametrize("bug", ["scaled before the max", "dropped last odd column"])
+def test_softmax_rows_bugs_are_caught(dtype, bug):
+    """exp(scale x - max x): the logits scaled before the unscaled maximum is subtracted, which overflows fp32 on a
+    negative-going row; the last column of an odd-width row never stored."""
+    scale, cols = 512 ** -0.5, 1025
+    s = _softmax_logits(4, cols, scale)
+    s[1] -= 3000.0  # a row far below zero
+    exact = ct.softmax_rows_ref(s, scale, dtype)
+    if bug == "scaled before the max":
+        e = torch.exp(s * ct._f32(scale) - s.amax(1, keepdim=True))  # fp32, as the kernel would compute it
+        mutated = (e / e.sum(1, keepdim=True)).double()
+    else:
+        mutated = exact[0].clone()
+        mutated[:, -1] = float("nan")
+    _caught(exact, mutated, dtype)
+
+
+def _moments(N=2, L=4, h=3, w=5, ld=64, seed=73):
+    g = torch.Generator().manual_seed(seed)
+    mom = torch.full((N * h * w, ld), float("nan"))
+    mom[:, :L] = torch.randn(N * h * w, L, generator=g) * 3
+    mom[:, L:2 * L] = torch.rand(N * h * w, L, generator=g) * 60 - 35  # logvar in [-35, 25): both clamp edges
+    return mom, torch.randn(N, L, h, w, generator=g)
+
+
+def test_gaussian_sample_ref_matches_diagonal_gaussian_sample():
+    """The diffusers formula (oracle DiagonalGaussianDistribution.sample with the given noise) times the scale, and
+    NaN in from either the mean or the logvar gives NaN out."""
+    from oracle.vae import DiagonalGaussianDistribution
+    mom, eps = _moments()
+    mom[3, 1], mom[7, 4 + 2] = float("nan"), float("nan")
+    N, L, h, w = eps.shape
+    params = mom[:, :2 * L].double().reshape(N, h, w, 2 * L).permute(0, 3, 1, 2)
+    want = DiagonalGaussianDistribution(params).sample(noise=eps.double()) * ct._f32(0.18215)
+    ref, bound = ct.gaussian_sample_ref(mom, mom.stride(0), eps, L, 0.18215)
+    assert torch.allclose(ref, want, rtol=1e-12, atol=0, equal_nan=True)
+    assert torch.isnan(ref).sum() == 2 and torch.equal(torch.isnan(ref), torch.isnan(bound))
+
+
+@pytest.mark.parametrize("bug", ["clamp at 30", "mean and logvar swapped", "NHWC output"])
+def test_gaussian_sample_bugs_are_caught(bug):
+    mom, eps = _moments()
+    N, L, h, w = eps.shape
+    exact = ct.gaussian_sample_ref(mom, mom.stride(0), eps, L, 0.18215)
+    if bug == "clamp at 30":
+        m4 = mom[:, :2 * L].double().reshape(N, h, w, 2 * L).permute(0, 3, 1, 2)
+        mutated = (m4[:, :L] + torch.exp(0.5 * m4[:, L:].clamp(-30.0, 30.0)) * eps.double()) * ct._f32(0.18215)
+    elif bug == "mean and logvar swapped":
+        sw = mom.clone()
+        sw[:, :L], sw[:, L:2 * L] = mom[:, L:2 * L], mom[:, :L]
+        mutated, _ = ct.gaussian_sample_ref(sw, sw.stride(0), eps, L, 0.18215)
+    else:
+        mutated = exact[0].permute(0, 2, 3, 1).reshape(exact[0].shape)
+    _caught(exact, mutated, torch.float32)
+
+
+def _mse_like_the_kernel(a, b):
+    """pf_mse_loss in fp32: 296 chunks, 256 thread-strided chains each, a shuffle tree, 8 warp partials in series,
+    then the fp64 sum of the partials and the fp64 mean rounded to fp32."""
+    n = a.numel()
+    chunk = -(-n // ct.MSE_CTAS)
+    k = -(-chunk // 256)
+    d = torch.zeros(ct.MSE_CTAS * chunk)
+    d[:n] = a.reshape(-1) - b.reshape(-1)
+    d = torch.nn.functional.pad(d.reshape(ct.MSE_CTAS, chunk), (0, k * 256 - chunk)).reshape(ct.MSE_CTAS, k, 256)
+    acc = torch.zeros(ct.MSE_CTAS, 256)
+    for i in range(k):
+        acc = acc + d[:, i] * d[:, i]
+    acc = acc.reshape(ct.MSE_CTAS, 8, 32)
+    for o in (16, 8, 4, 2, 1):
+        acc = acc[..., :o] + acc[..., o:2 * o]
+    s = torch.zeros(ct.MSE_CTAS)
+    for wi in range(8):
+        s = s + acc[:, wi, 0]
+    return torch.tensor(float(s.double().sum() / n), dtype=torch.float32)
+
+
+@pytest.mark.parametrize("n", [100, 296 * 37 - 1, 296 * 443 + 1])
+def test_mse_ref_matches_torch_and_catches_the_padded_count(n):
+    """mse_ref equals F.mse_loss; the kernel's fp32 summation order passes its bound; a mean over the padded count
+    296 * ceil(n / 296) fails it."""
+    g = torch.Generator().manual_seed(n)
+    a, b = torch.randn(n, generator=g) * 2 + 0.5, torch.randn(n, generator=g)
+    ref, bound = ct.mse_ref(a, b)
+    assert torch.allclose(ref, torch.nn.functional.mse_loss(a.double(), b.double()), rtol=1e-13, atol=0)
+    assert abs(_mse_like_the_kernel(a, b).double() - ref) <= bound
+    assert abs(ref.float().double() - ref) <= bound
+    padded = (a.double() - b.double()).pow(2).sum() / (ct.MSE_CTAS * -(-n // ct.MSE_CTAS))
+    assert abs(padded.float().double() - ref) > bound

@@ -1,7 +1,8 @@
-"""-m gpu: conv_in, the panorama branch's conv_out and copy2d against plain PyTorch fp32 on the same 16-bit-rounded
-inputs, pad_pano bit for bit, and the EPPA tables against the oracle's get_masks / get_coords / SphericalPE
-(models/pano/utils.py:10-106, transformer.py:185-201). GroupNorm, LayerNorm, CFG + DDIM and the timestep embedding are
-held to their fp64 contracts in test_gpu_norm_contract.py."""
+"""-m gpu: the panorama branch's conv_out and copy2d (pf_copy2d) against plain PyTorch fp32 on the same 16-bit-rounded
+inputs, pad_pano (pf_pad_pano) bit for bit, and the EPPA tables (pf_eppa_tables, pf_eppa_pe) against the oracle's
+get_masks / get_coords / SphericalPE (models/pano/utils.py:10-106, transformer.py:185-201). conv_in is held to its fp64
+contract in test_gpu_elementwise_contract.py; GroupNorm, LayerNorm, CFG + DDIM and the timestep embedding in
+test_gpu_norm_contract.py."""
 from types import SimpleNamespace
 
 import numpy as np
@@ -13,18 +14,13 @@ pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("circ", [False, True])
-def test_conv_in_and_branch_conv_out(cuda_device, circ):
-    from panfusion_b200 import engine, ops
+def test_branch_conv_out(cuda_device, circ):
+    from panfusion_b200 import engine
     from panfusion_b200.packing import pack_conv3x3
     from oracle.eppa import pad_pano, unpad_pano
     g = torch.Generator().manual_seed(4)
     N, H, W, C = 2, 16, 32, 320
-    lat = torch.randn(N, 4, H, W, generator=g)
-    w_in, b_in = torch.randn(C, 4, 3, 3, generator=g) * 0.2, torch.randn(C, generator=g)
     conv = lambda x, w, b: unpad_pano(F.conv2d(pad_pano(x, 1), w, b, padding=1), 1) if circ else F.conv2d(x, w, b, padding=1)
-    ref = conv(lat, w_in, b_in)
-    got = ops.conv_in(lat.to(cuda_device), w_in.to(cuda_device), b_in.to(cuda_device), torch.float16, circ)
-    torch.testing.assert_close(got.float().cpu().reshape(N, H, W, C).permute(0, 3, 1, 2), ref, rtol=1e-3, atol=2e-3)
     # conv_norm_out -> SiLU -> conv_out, as Branch.conv_out runs it: pf_gn_prep, then the 64-wide tap-GEMM
     x = torch.randn(N, C, H, W, generator=g).half()
     gamma, beta = torch.randn(C, generator=g), torch.randn(C, generator=g)
@@ -41,24 +37,6 @@ def test_conv_in_and_branch_conv_out(cuda_device, circ):
     got = br.conv_out(engine.img_from_nchw(x.to(cuda_device), torch.float16))
     # the prepared activations and the packed weights are rounded to fp16
     torch.testing.assert_close(got.cpu(), ref, rtol=2e-3, atol=3e-3)
-
-
-@pytest.mark.parametrize("W", [32, 30])  # 4-pixel register-blocked path and the generic one
-def test_conv_in_silu_layout_image(cuda_device, W):
-    """pf_conv_in with act = SiLU on a 3-channel image: first conv of the ControlNet conditioning embedding, output
-    channels zero-padded 16 -> 64 (padded channels must come out exactly 0 = silu(0))."""
-    from panfusion_b200 import ops
-    g = torch.Generator().manual_seed(9)
-    N, H = 2, 24
-    img = torch.rand(N, 3, H, W, generator=g)
-    w, b = torch.randn(16, 3, 3, 3, generator=g) * 0.3, torch.randn(16, generator=g)
-    ref = F.silu(F.conv2d(img, w, b, padding=1))
-    wp, bp = torch.zeros(64, 3, 3, 3), torch.zeros(64)
-    wp[:16], bp[:16] = w, b
-    got = ops.conv_in(img.to(cuda_device), wp.to(cuda_device), bp.to(cuda_device), torch.float16, False,
-                      act=ops.PF_ACT_SILU).float().cpu().reshape(N, H, W, 64).permute(0, 3, 1, 2)
-    torch.testing.assert_close(got[:, :16], ref, rtol=1e-3, atol=1e-3)
-    assert got[:, 16:].abs().max().item() == 0.0
 
 
 def test_copy2d(cuda_device):
